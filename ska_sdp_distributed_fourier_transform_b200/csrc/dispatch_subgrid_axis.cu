@@ -75,6 +75,10 @@ static int launch_sg_axis_pp(const swiftly_b200* h, const SubgridAxisArgs& a, cu
     // accumulator.  Measured slower: the group barrier it needs before the
     // round's stores re-aligns the transforms that the split-exchange form lets drift apart.
     k.cx_round0 = (h->sg_variant == 16 && XM == (XM / M) * M && M > 16) ? 1 : 0;
+    // sg_variant 25: the former round scheme -- transform slots without a source transform
+    // zeros, and the accumulator is cleared ahead of the rounds unless the first round tiles it
+    // (tools/quick_k3.py compares it with the default)
+    k.compute_empty = h->sg_variant == 25 ? 1 : 0;
     // (the last box may be partial: the engine still reads a whole box from shared memory)
     const size_t staged = (size_t)((a.sz + k.tma_box - 1) / (k.tma_box > 0 ? k.tma_box : 1)) *
                           (size_t)k.tma_box * sizeof(cplx);

@@ -49,6 +49,9 @@ struct SubgridAxisKernelPP {
 #endif
     // named barriers need whole warps; smaller transforms use the group barrier
     static constexpr bool SUB_BARRIERS = (T_M % 32 == 0) && CONC > 1;
+    // a slot without a source can sit its round out only when its transform's barriers are its
+    // own (with the group barrier or the token every slot has to take part in every exchange)
+    static constexpr bool CAN_SKIP = SUB_BARRIERS && !TOKENS;
 
     // identical to SubgridAxisKernel
     SgSource src[SW_MAX_SOURCES];
@@ -77,6 +80,9 @@ struct SubgridAxisKernelPP {
     int cx_round0;                     // first round exchanges complex samples in the accumulator
     int pf_mode;                       // L2 prefetch: 0 bulk at the first exchange (default),
                                        // 1 none, 2 per-thread prefetch at the start of the round
+    int compute_empty;                 // empty slots transform zeros and the accumulator is
+                                       // cleared first unless the first round tiles it (the
+                                       // former scheme, kept to compare against)
     cplx* out_g[SW_MAX_GROUPS];        // optional per-group output base (null: out + g * out_gs)
     // tensor maps travel as a separate __grid_constant__ kernel parameter (ctx.tmaps)
     struct Maps {
@@ -110,14 +116,31 @@ struct SubgridAxisKernelPP {
             if (order_stores) ctx.group_sync(1 + grp, T_X);
         }
         SW_HD void operator()() const { ctx.group_sync(bar_id, bar_count); }
-        // start of an exchange phase: with TOKENS wait for the token (the other group's
-        // release); either way a barrier over (at least) the transform's threads
-        SW_HD void acquire() {
+        SW_HD void prefetch() {
             if (pf_bytes[0]) {
                 ctx.bulk_prefetch_l2(pf_ptr[0], pf_bytes[0]);
                 if (pf_bytes[1]) ctx.bulk_prefetch_l2(pf_ptr[1], pf_bytes[1]);
                 pf_bytes[0] = pf_bytes[1] = 0;
             }
+        }
+        // a transform slot without a source in this round (no TOKENS): what the slot's threads
+        // owe the rest of the group when they skip the transform -- the L2 prefetch of the
+        // slot's next window and, after a line that left through the TMA engine, the wait for
+        // the bulk stores together with the group-wide barrier of the first exchange.  The
+        // transform's own barriers (3 + g * CONC + c) involve nobody else and are skipped; the
+        // caller still owes pre_store().
+        SW_HD void idle() {
+            prefetch();
+            if (tma_pending) {
+                tma_pending = false;
+                if (t == 0) ctx.bulk_wait_read();
+                ctx.group_sync(1 + grp, T_X);
+            }
+        }
+        // start of an exchange phase: with TOKENS wait for the token (the other group's
+        // release); either way a barrier over (at least) the transform's threads
+        SW_HD void acquire() {
+            prefetch();
             if (tma_pending) {
                 tma_pending = false;
                 if (t == 0) ctx.bulk_wait_read();
@@ -144,6 +167,9 @@ struct SubgridAxisKernelPP {
         double* work = (double*)((cplx*)ctx.smem + (size_t)GROUPS * ACCS) + (size_t)grp * WORK;
         const int c = t / T_M;
         const int lt = t % T_M;
+        // slots without a source sit their round out (a sparse facet cover leaves up to three
+        // of four slots of a round empty; otherwise they transform zeros)
+        const bool skip_empty = CAN_SKIP && !compute_empty;
         GroupSync<Ctx> gsync{ctx, 1 + grp, T_X, grp, t, false, {nullptr, nullptr}, {0, 0}, false};
         GroupSync<Ctx> msync{ctx, SUB_BARRIERS ? 3 + grp * CONC + c : 1 + grp,
                              SUB_BARRIERS ? T_M : T_X, grp, t, false, {nullptr, nullptr}, {0, 0},
@@ -173,14 +199,26 @@ struct SubgridAxisKernelPP {
             // the previous line's bulk stores must have read the staging (= work) buffer before
             // the first exchange THROUGH THE WORK AREA writes it (see GroupSync::acquire)
             bool tma_wait_due = tma_out != 0;
-            if (!first_round_tiles) {
+            if (!skip_empty && !first_round_tiles) {
                 for (int i = t; i < XM; i += T_X) acc[i] = mk(0.0, 0.0);
                 gsync();
             }
             for (int slot0 = 0; slot0 < n_slots; slot0 += CONC) {
-                const bool overwrite = first_round_tiles && slot0 == 0;
+                // Which transforms of the round have a source (the same answer in every thread
+                // of the group).  The windows of a round are pairwise disjoint, so the first
+                // round stores instead of accumulating; the accumulator positions that no
+                // window of the first round covers are cleared by the threads of its empty
+                // slots, before the pre-store barrier of the next round (or the barrier ahead
+                // of the xM-point transform).  CONC * M == XM: a first round without an empty
+                // slot tiles the accumulator.
+                unsigned act = 0;
+#pragma unroll
+                for (int k = 0; k < CONC; ++k)
+                    if (line_ok && slot0 + k < n_slots && src[sgrp * n_slots + slot0 + k].base != nullptr)
+                        act |= 1u << k;
+                const bool overwrite = skip_empty ? slot0 == 0 : (first_round_tiles && slot0 == 0);
                 const int slot = sgrp * n_slots + slot0 + c;
-                const bool active = line_ok && slot0 + c < n_slots && src[slot].base != nullptr;
+                const bool active = (act >> c) & 1u;
                 const cplx* base = active ? src[slot].base + line * src[slot].ls : nullptr;
                 const int64_t es = active ? src[slot].es : 0;
                 const int wbase = active ? src[slot].wbase : 0;
@@ -244,11 +282,42 @@ struct SubgridAxisKernelPP {
                         }
                     }
                 }
-                if (tma_wait_due && !(overwrite && cx_round0)) {
+                if (skip_empty && act == 0) {
+                    // no transform in this round (a group with fewer rounds than the launch,
+                    // a line past the end): the first round leaves a cleared accumulator
+                    msync.prefetch();
+                    if (slot0 == 0)
+                        for (int i = t; i < XM; i += T_X) acc[i] = mk(0.0, 0.0);
+                    continue;
+                }
+                const bool cx = overwrite && cx_round0 && (!skip_empty || act == (1u << CONC) - 1);
+                if (tma_wait_due && !cx) {
                     msync.tma_pending = true;
                     tma_wait_due = false;
                 }
-                if (overwrite && cx_round0) {
+                if (skip_empty && !active) {
+                    msync.idle();
+                    if (overwrite) {
+                        // the first round's uncovered positions, shared by its empty slots
+                        int rank = 0, n_idle = 0;
+#pragma unroll
+                        for (int k = 0; k < CONC; ++k)
+                            if (!((act >> k) & 1u)) {
+                                rank += k < c;
+                                ++n_idle;
+                            }
+                        for (int i = rank * T_M + lt; i < XM; i += n_idle * T_M) {
+                            bool covered = false;
+#pragma unroll
+                            for (int k = 0; k < CONC; ++k)
+                                if ((act >> k) & 1u)
+                                    covered |= wrap_sub(i, src[sgrp * n_slots + slot0 + k].pos_base, XM) < M;
+                            if (!covered) acc[i] = mk(0.0, 0.0);
+                        }
+                    }
+                    msync.order_stores = slot0 > 0;
+                    msync.pre_store();
+                } else if (cx) {
                     // First round of a tiling layout: the accumulator holds nothing yet, so its
                     // storage serves as COMPLEX exchange buffers of the round's transforms (one
                     // trip, two barriers per pass instead of two trips and four; CONC * (M +
