@@ -218,7 +218,9 @@ int swiftly_b200_fold_column(const swiftly_b200* plan, int n_facets,
                              const swiftly_b200_lines* facet_accs, const int64_t* facet_off1,
                              const double* const* mask1, int64_t subgrid_off0, void* stream);
 
-/* xM_size / xM_yN_size if the fused kernel exists for this plan, else 0. */
+/* xM_size / xM_yN_size (1, 2, 3, 4 or 8: the sources one round of the fused kernel adds) if the
+ * fused kernel exists for this plan, else 0.  It exists for every (xM_yN_size, xM_size) pair of
+ * the parameter catalogue. */
 int swiftly_b200_sum_finish_axis_supported(const swiftly_b200* plan);
 
 #ifdef __cplusplus

@@ -50,17 +50,22 @@ static cplx unit_root(long double num, long double den) {  // exp(-2 pi i num / 
 
 // Compact per-pass table of the n-point Stockham plan (fft_engine.cuh): for every pass
 // after the first, with sub-transform size Ns (16, 256, 4096) and radix R, the Ns entries
-// exp(-2 pi i k / (Ns R)), k < Ns, stored pass after pass.
+// exp(-2 pi i k / (Ns R)), k < Ns, stored pass after pass.  A mixed-radix length n = F * p
+// (p the power-of-two part, line_fft_mixed in fft_engine.cuh) gets the table of the p-point
+// plan followed by exp(-2 pi i t / n), t < n.
 const cplx* twiddles(const swiftly_b200* h, int n) {
     std::lock_guard<std::mutex> lock(h->mu);
     auto it = h->tw.find(n);
     if (it != h->tw.end()) return it->second;
     std::vector<cplx> host;
-    for (int ns = 16; ns < n; ns *= 16) {
-        const int r = (n / ns >= 16) ? 16 : n / ns;
+    const int p = n & -n;
+    for (int ns = 16; ns < p; ns *= 16) {
+        const int r = (p / ns >= 16) ? 16 : p / ns;
         for (int k = 0; k < ns; ++k) host.push_back(unit_root(k, (long double)ns * r));
     }
     if (host.empty()) host.push_back(unit_root(0, 1));
+    if (p != n)
+        for (int t = 0; t < n; ++t) host.push_back(unit_root(t, n));
     return upload_table(h, n, host);
 }
 

@@ -234,10 +234,22 @@ struct DeviceCtx {
 
 extern __shared__ __align__(1024) char swiftly_dyn_smem[];
 
-// register budget: at least 512 resident threads per SM (<= 128 registers/thread)
+// A body may declare WARP_BOUNDS = true: its CTAs are not whole warps (e.g. 10..28 threads),
+// and the register budget below then counts the warps the hardware allocates for them.
+template <class Body, class = void>
+struct WarpBounds : std::false_type {};
+template <class Body>
+struct WarpBounds<Body, std::void_t<decltype(Body::WARP_BOUNDS)>>
+    : std::integral_constant<bool, Body::WARP_BOUNDS> {};
+
+// register budget: at least 512 resident threads per SM (<= 128 registers/thread).  Registers
+// are allocated per warp, so a CTA of fewer than 32 threads costs a whole warp's registers:
+// counted by thread, 512 / 16 = 32 such CTAs would hold 1024 threads' worth and cap them at 64.
 template <class Body>
 struct MinBlocks {
-    static constexpr int V = Body::THREADS >= 512 ? 1 : 512 / Body::THREADS;
+    static constexpr int ALLOC = WarpBounds<Body>::value ? (Body::THREADS + 31) / 32 * 32
+                                                         : Body::THREADS;
+    static constexpr int V = ALLOC >= 512 ? 1 : 512 / ALLOC;
 };
 
 template <class Body>

@@ -28,7 +28,9 @@ static int launch_sg_axis_l(const swiftly_b200* h, const SubgridAxisArgs& a, cud
     k.scale = 1.0 / (double)XM;
     k.first_round_tiles = a.first_round_tiles;
     k.accumulate_out = a.accumulate_out;
-    cudaError_t e = launch_body(k, grid_for(((a.n_lines + LINES - 1) / LINES) * a.n_groups, 1), k.SMEM, s);
+    int grid = grid_for(((a.n_lines + LINES - 1) / LINES) * a.n_groups, 1);
+    if (h->max_blocks > 0 && grid > h->max_blocks) grid = h->max_blocks;  // (test hook)
+    cudaError_t e = launch_body(k, grid, k.SMEM, s);
     return e == cudaSuccess ? SWIFTLY_B200_OK : cuda_fail(e, "subgrid axis kernel launch");
 }
 
@@ -109,12 +111,16 @@ static int launch_sg_axis_pp(const swiftly_b200* h, const SubgridAxisArgs& a, cu
     return e == cudaSuccess ? SWIFTLY_B200_OK : cuda_fail(e, "subgrid axis (two-group) kernel launch");
 }
 
+// The two-group kernel takes power-of-two lengths with CONC = 2 or 4.  The catalogue's other
+// pairs run the round-1 kernel: CONC = 8 (m = 128, xM = 1024: eight-thread transforms), CONC = 1
+// (m = xM = 256: one source per round) and the mixed-radix lengths (3, 5, 7 * 2^k).
 template <int M, int XM>
 struct PingPongFits {
+    static constexpr bool POW2 = (M & (M - 1)) == 0 && (XM & (XM - 1)) == 0 && XM / M >= 2;
 #if defined(SWIFTLY_EMU)
-    static constexpr bool V = (XM / M) <= 4;
+    static constexpr bool V = POW2 && (XM / M) <= 4;
 #else
-    static constexpr bool V = (XM / M) <= 4 && (XM / 16) % 32 == 0 &&
+    static constexpr bool V = POW2 && (XM / M) <= 4 && (XM / 16) % 32 == 0 &&
                               2 * ((size_t)(XM + XM / 16) * 16 + (size_t)(XM + XM / 16 + 24) * 8) <=
                                   227 * 1024;
 #endif
@@ -136,15 +142,18 @@ static int launch_sg_axis(const swiftly_b200* h, const SubgridAxisArgs& a, cudaS
     }
     // 2 lines need 2 x (acc + work) of shared memory: only the pairs that fit
     if constexpr (2 * ((size_t)(XM + 4) * sizeof(cplx) + (size_t)(XM + XM / 16 + 40) * 8) <=
-                  227 * 1024) {
+                      227 * 1024 &&
+                  SubgridAxisKernel<M, XM, 2>::SMEM <= 227 * 1024) {
         if (adjacent) return launch_sg_axis_l<M, XM, 2>(h, a, s);
     }
     return launch_sg_axis_l<M, XM, 1>(h, a, s);
 }
 
+// the last six: the catalogue pairs outside xM / m in {2, 4} (swift_configs.json)
 #define SW_SG_PAIRS(X) \
     X(32, 64) X(32, 128) X(64, 128) X(64, 256) X(128, 256) X(128, 512) X(256, 512) X(256, 1024) \
-    X(512, 1024) X(512, 2048) X(1024, 2048) X(1024, 4096) X(2048, 4096) X(2048, 8192)
+    X(512, 1024) X(512, 2048) X(1024, 2048) X(1024, 4096) X(2048, 4096) X(2048, 8192)         \
+    X(128, 1024) X(256, 256) X(128, 384) X(160, 320) X(192, 384) X(224, 448)
 
 int subgrid_axis_conc(int m, int xM) {
 #define X(M, XM) if (m == M && xM == XM) return XM / M;

@@ -431,4 +431,90 @@ SW_HD void line_fft_cx(int lt, cplx* sm, const cplx* tw, Ld& ld, St& st, Sync& s
     stockham_tail_cx<N, R, R, DIR>(lt, sm, tw, v, st, sync);
 }
 
+// ---------------------------------------------------------------- mixed-radix lines
+// Lengths N = F * P with F in {3, 5, 7} and P a power of two >= 32 (the xM and m of the
+// catalogue's non power-of-two geometries: 320, 384, 448 and 160, 192, 224), still with
+// T = N / 16 threads per line.  Decimation in time by F, all in shared memory:
+//   E_q = FFT_P(z[F j + q]),  q < F      (F concurrent P-point transforms, P / 16 threads each)
+//   X[o] = sum_q w^(q o) E_q[o mod P],  w = exp(DIR 2 pi i / N)
+// (the split-F decomposition of the line kernels, SplitFKernel in kernels.cuh, with the
+// sub-transform outputs kept in the line's work area instead of the L2 scratch).  Every thread
+// combines 16 outputs o = lt + i * T: F - 1 complex multiplies each, twiddles from the table
+// exp(-2 pi i t / N), t < N, that follows the P-point plan's compact table in `tw`.
+// Work area (doubles): F exchange buffers of the P-point transforms, then the F * P outputs E.
+template <int N, bool POW2 = (N & (N - 1)) == 0>
+struct LineCfg {  // power of two: the Stockham plan of FftCfg
+    static constexpr int T = FftCfg<N>::T;
+    static constexpr int SCRATCH = FftCfg<N>::PADDED;  // doubles of work area per line
+};
+
+constexpr int odd_part(int n) { return n % 2 ? n : odd_part(n / 2); }
+
+// entries of the compact per-pass table of the P-point plan (twiddles() in capi.cu)
+constexpr int compact_tw_size(int p) {
+    int s = 0;
+    for (int ns = 16; ns < p; ns *= 16) s += ns;
+    return s ? s : 1;
+}
+
+template <int N>
+struct LineCfg<N, false> {
+    static constexpr int F = odd_part(N);
+    static constexpr int P = N / F;
+    static_assert(F == 3 || F == 5 || F == 7, "mixed-radix lines: N = F * 2^k, F in {3, 5, 7}");
+    static_assert(P >= 32 && P <= 8192, "mixed-radix lines: 32 <= 2^k <= 8192");
+    static constexpr int T = N / 16;
+    static constexpr int TP = P / 16;                     // threads per P-point transform
+    static constexpr int XSTRIDE = FftCfg<P>::PADDED | 1;  // odd: the exchanges hit other banks
+    static constexpr int EOFF = (F * XSTRIDE + 1) & ~1;   // E is complex: 16-byte aligned
+    static constexpr int SCRATCH = EOFF + 2 * N;
+    static constexpr int TW_FULL = compact_tw_size(P);    // offset of exp(-2 pi i t / N) in tw
+};
+
+// Mixed-radix line (see LineCfg<N, false>).  Same arguments as line_fft; `sm` holds
+// LineCfg<N>::SCRATCH doubles; sync() is a plain barrier over (at least) the line's threads.
+// The storer is called as st(o, v) or st(o, v, i, 0) with o = lt + i * T.
+template <int N, int DIR, class Ld, class St, class Sync>
+SW_HD void line_fft_mixed(int lt, double* sm, const cplx* tw, Ld& ld, St& st, Sync& sync) {
+    typedef LineCfg<N> C;
+    constexpr int F = C::F, P = C::P;
+    static_assert(!HasPhaseHooks<Sync>::value, "mixed-radix lines take a plain barrier");
+    const int q = lt / C::TP;
+    cplx* e = (cplx*)(sm + C::EOFF);
+    {
+        auto ldq = [&](int j) { return ld(F * j + q); };
+        cplx* eq = e + q * P;
+        auto stq = [&](int k, cplx v) { eq[k] = v; };
+        line_fft<P, DIR>(lt - q * C::TP, sm + q * C::XSTRIDE, tw, ldq, stq, sync);
+    }
+    sync();  // every E_q complete
+    const cplx* wn = tw + C::TW_FULL;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+        const int o = lt + i * C::T;
+        const int k = o & (P - 1);
+        cplx x = e[k];
+        int t = 0;  // q * o mod N
+#pragma unroll
+        for (int qq = 1; qq < F; ++qq) {
+            t += o;
+            if (t >= N) t -= N;
+            cplx w = ldg_c(wn + t);
+            if (DIR > 0) w.y = -w.y;
+            x = cadd(x, cmul(e[qq * P + k], w));
+        }
+        call_store(st, o, x, i, 0);
+    }
+}
+
+// line_fft for every length the fused subgrid kernels take: the Stockham plan for powers of
+// two, the mixed-radix line otherwise (work area: LineCfg<N>::SCRATCH doubles)
+template <int N, int DIR, class Ld, class St, class Sync>
+SW_HD void line_fft_any(int lt, double* sm, const cplx* tw, Ld& ld, St& st, Sync& sync) {
+    if constexpr ((N & (N - 1)) == 0)
+        line_fft<N, DIR>(lt, sm, tw, ld, st, sync);
+    else
+        line_fft_mixed<N, DIR>(lt, sm, tw, ld, st, sync);
+}
+
 }  // namespace swiftly

@@ -628,20 +628,33 @@ struct SgSource {
 // lanes (lane pairs touch 32 contiguous bytes): used when lines are adjacent in memory
 // (axis-0 work on C-ordered arrays), where one line per CTA would fetch every 32-byte
 // sector twice.
+//
+// m and xM may also be mixed-radix lengths (LineCfg<N, false> in fft_engine.cuh, the
+// catalogue's 3, 5 and 7 * 2^k geometries); the transforms then go through line_fft_mixed,
+// whose work area also holds the sub-transform outputs.
 template <int M, int XM, int LINES>
 struct SubgridAxisKernel {
-    static constexpr int T_M = FftCfg<M>::T;
-    static constexpr int T_X = FftCfg<XM>::T;
+    static constexpr int T_M = LineCfg<M>::T;
+    static constexpr int T_X = LineCfg<XM>::T;
     static constexpr int THREADS = T_X * LINES;
     static constexpr int CONC = T_X / T_M;  // = XM / M concurrent m-point transforms per line
-    static constexpr int WSTRIDE = FftCfg<M>::PADDED | 1;
-    static constexpr int WORK0 = CONC * WSTRIDE;  // doubles, >= FftCfg<XM>::PADDED
-    static_assert(WORK0 >= FftCfg<XM>::PADDED, "work area must hold the xM exchange buffer");
+    // power of two: odd stride (the transforms' exchanges land in different banks); mixed
+    // radix: even (the work area holds complex samples)
+    static constexpr int WSTRIDE = (M & (M - 1)) == 0 ? (LineCfg<M>::SCRATCH | 1)
+                                                      : ((LineCfg<M>::SCRATCH + 1) & ~1);
+    // doubles: the CONC m-point work areas, which the xM-point transform reuses
+    static constexpr int WORK0 = CONC * WSTRIDE >= LineCfg<XM>::SCRATCH ? CONC * WSTRIDE
+                                                                         : LineCfg<XM>::SCRATCH;
     // per-line strides: the second line lands 8 bank pairs (64 B) away from the first
     static constexpr int WORK = LINES == 1 ? WORK0 : ((WORK0 + 15) / 16) * 16 + 8;
     static constexpr int ACCS = LINES == 1 ? XM : XM + 4;
     static constexpr size_t SMEM =
         ((size_t)ACCS * sizeof(cplx) + (size_t)WORK * sizeof(double)) * LINES;
+    // register budget by allocated warps (MinBlocks, common.cuh) for the pairs added for the
+    // catalogue whose CTAs are not whole warps: the mixed-radix lengths and m = xM = 256
+    // (10..56 threads).  Counted by thread their budget was 64..96 registers and they spilled
+    // 380..908 bytes.  The earlier power-of-two pairs keep the budget they were measured with.
+    static constexpr bool WARP_BOUNDS = (M & (M - 1)) != 0 || (XM & (XM - 1)) != 0 || M == XM;
 
     // Several independent "groups" (e.g. the facet rows of one subgrid) share one launch:
     // group g uses source slots [g * n_slots, (g + 1) * n_slots), has n_lines lines and
@@ -755,7 +768,7 @@ struct SubgridAxisKernel {
                         }
                     }
                 }
-                line_fft<M, -1>(lt, work + (size_t)c * WSTRIDE, tw_m, ld, st, gsync);
+                line_fft_any<M, -1>(lt, work + (size_t)c * WSTRIDE, tw_m, ld, st, gsync);
                 ctx.sync();
             }
             {
@@ -777,7 +790,7 @@ struct SubgridAxisKernel {
                         }
                     }
                 };
-                line_fft<XM, +1>(t, work, tw_x, ld, st, sync);
+                line_fft_any<XM, +1>(t, work, tw_x, ld, st, sync);
             }
             ctx.sync();  // acc / work are reused by the next line
         }

@@ -10,9 +10,14 @@ Named SwiFTly parameter sets (``SWIFT_CONFIGS[name]`` -> ``SwiftlyConfig`` keywo
 ``runnable(params)`` tells whether this build can transform a set: every FFT length
 (``yN_size``, ``xM_size``, ``xM_size*yN_size/N``) must be ``F * 2^k`` with ``F <= 16`` and
 ``16 <= 2^k <= 8192`` -- true for all 244 catalogue entries (factors 3, 5, 7, 9 and lengths up
-to 65536 go through the generic split-F kernel; the fused forward kernels cover the
-power-of-two sets, the others run primitive by primitive on the GPU).  Anything else raises
+to 65536 go through the generic split-F kernel).  Anything else raises
 ``NotImplementedError`` when a transform is requested.
+
+``fused_forward(params)`` tells whether the fused forward kernels (``sum_finish_axis``) exist
+for the set's ``(m, xM)`` pair, ``m = xM_size * yN_size / N``.  They do for every catalogue
+entry: power-of-two pairs with ``xM / m`` in {1, 2, 4, 8}, and the mixed-radix pairs
+(128, 384), (160, 320), (192, 384), (224, 448).  Other runnable sets take the forward path
+primitive by primitive.
 """
 
 import json
@@ -64,9 +69,16 @@ def runnable(params):
     return all(fft_length_supported(s) for s in (yN, xM, xM * yN // N))
 
 
+# (m, xM) pairs with a fused subgrid kernel: SW_SG_PAIRS in csrc/dispatch_subgrid_axis.cu
+FUSED_FORWARD_PAIRS = frozenset([
+    (32, 64), (32, 128), (64, 128), (64, 256), (128, 256), (128, 512), (256, 512), (256, 1024),
+    (512, 1024), (512, 2048), (1024, 2048), (1024, 4096), (2048, 4096), (2048, 8192),
+    (128, 1024), (256, 256), (128, 384), (160, 320), (192, 384), (224, 448),
+])
+
+
 def fused_forward(params):
-    """True if the fused forward kernels (power-of-two m, xM with xM/m in {2, 4}) apply."""
+    """True if the fused forward kernels exist for the set's ``(m, xM)`` pair (every catalogue
+    entry; see the module docstring)."""
     N, yN, xM = params["N"], params["yN_size"], params["xM_size"]
-    m = xM * yN // N
-    pow2 = lambda v: v & (v - 1) == 0  # noqa: E731
-    return pow2(m) and pow2(xM) and xM // m in (2, 4) and 32 <= m <= 2048 and xM <= 8192
+    return (xM * yN // N, xM) in FUSED_FORWARD_PAIRS
