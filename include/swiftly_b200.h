@@ -223,6 +223,43 @@ int swiftly_b200_fold_column(const swiftly_b200* plan, int n_facets,
  * the parameter catalogue. */
 int swiftly_b200_sum_finish_axis_supported(const swiftly_b200* plan);
 
+/* One output of swiftly_b200_split_subgrid_axis: n_lines lines (the input's line count),
+ * sample (l, i) at data[l * line_stride + i * elem_stride] (complex elements). */
+typedef struct swiftly_b200_split_target {
+    void* data; /* device pointer */
+    int64_t n_lines;
+    int64_t line_stride;
+    int64_t elem_stride;
+    int64_t facet_off; /* facet offset along the transformed axis */
+} swiftly_b200_split_target;
+
+#define SWIFTLY_B200_SPLIT_STORE 0 /* targets: xM_yN_size samples per line, overwritten    */
+#define SWIFTLY_B200_SPLIT_ADD 1   /* targets: yN_size samples per line, ACCUMULATED into  */
+
+/* The subgrid side of the backward transform along one axis in one kernel, the adjoint of
+ * swiftly_b200_sum_finish_axis.  For every line of inputs[g] (n_lines lines of size <=
+ * xM_size samples, the same n_lines in every group): prepare_subgrid along this axis with
+ * subgrid_offs[g] (core.py:328-368), kept in shared memory, then for every target of the group
+ * extract_from_subgrid(., facet_off) (core.py:370-406).
+ *   SWIFTLY_B200_SPLIT_STORE: the xM_yN_size contribution samples are stored (a strip line).
+ *   SWIFTLY_B200_SPLIT_ADD: they are added at the subgrid's position of a yN_size facet column
+ *     accumulator line: add_to_facet(., subgrid_offs[g]) (core.py:408-449; together
+ *     api_helper.py:115-152, extract_from_subgrid + accumulate_column).
+ * Group g takes targets [sum(group_sizes[:g]), ... + group_sizes[g]).  Targets only read the
+ * prepared line: their windows may overlap or repeat.  In add mode the targets of ONE group must
+ * be distinct accumulators; targets of different groups may share one (groups are applied in
+ * order, every line by one CTA: no atomics, deterministic sums).  Any number of groups and
+ * targets (larger jobs are cut into several launches).  Offsets are taken modulo N.  Returns
+ * SWIFTLY_B200_EUNSUPPORTED when swiftly_b200_split_axis_supported(plan) is 0. */
+int swiftly_b200_split_subgrid_axis(const swiftly_b200* plan, const swiftly_b200_lines* inputs,
+                                    int n_groups, const int64_t* subgrid_offs,
+                                    const swiftly_b200_split_target* targets,
+                                    const int32_t* group_sizes, int mode, void* stream);
+/* xM_size / xM_yN_size (at least 1: the targets one round transforms) if the fused split kernel
+ * exists for this plan, else 0; non-zero exactly for the pairs of
+ * swiftly_b200_sum_finish_axis_supported. */
+int swiftly_b200_split_axis_supported(const swiftly_b200* plan);
+
 #ifdef __cplusplus
 }
 #endif

@@ -48,6 +48,21 @@ class Source(ctypes.Structure):
     ]
 
 
+class SplitTarget(ctypes.Structure):
+    """``swiftly_b200_split_target``: one output of the fused subgrid split kernel."""
+
+    _fields_ = [
+        ("data", ctypes.c_void_p),
+        ("n_lines", ctypes.c_int64),
+        ("line_stride", ctypes.c_int64),
+        ("elem_stride", ctypes.c_int64),
+        ("facet_off", ctypes.c_int64),
+    ]
+
+
+SPLIT_STORE = 0
+SPLIT_ADD = 1
+
 _PLAN = ctypes.c_void_p
 _LINES_P = ctypes.POINTER(Lines)
 _D_P = ctypes.POINTER(ctypes.c_double)
@@ -85,6 +100,8 @@ SYMBOLS = {
     "swiftly_b200_subgrid_to_facets": (ctypes.c_int, [_PLAN, ctypes.c_int, _LINES_P, _LINES_P, ctypes.POINTER(ctypes.c_int64), ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_fold_column": (ctypes.c_int, [_PLAN, ctypes.c_int, _LINES_P, _LINES_P, ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_void_p), ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_sum_finish_axis_supported": (ctypes.c_int, [_PLAN]),
+    "swiftly_b200_split_subgrid_axis": (ctypes.c_int, [_PLAN, _LINES_P, ctypes.c_int, ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(SplitTarget), ctypes.POINTER(ctypes.c_int32), ctypes.c_int, ctypes.c_void_p]),
+    "swiftly_b200_split_axis_supported": (ctypes.c_int, [_PLAN]),
 }
 
 _lock = threading.Lock()

@@ -512,13 +512,26 @@ class SwiftlyBackward:
         # axis 0); otherwise the reference's task bodies run primitive by primitive
         self._fused = bool(hasattr(self.core, "subgrid_to_facets")
                            and getattr(self.core, "fused_backward_supported", lambda: False)())
+        # the subgrid side as two split kernels per subgrid (K4T along axis 0 into one strip
+        # per facet row, K3T along axis 1 into the column accumulators); the prepared subgrid
+        # and the (m, xM) blocks of the primitive chain never exist
+        self._split = self._fused and bool(
+            getattr(self.core, "split_axis_supported", lambda: False)())
+        rows = collections.OrderedDict()
+        for idx, cfg in enumerate(self.facets_config_list):
+            rows.setdefault(cfg.off0, []).append(idx)
+        self._rows = list(rows.items())
+        self._row_members = dict(self._rows)
+        self._strips = None
         self._masks1 = None
 
     def add_new_subgrid_task(self, subgrid_config, new_subgrid_task):
         """Fold one subgrid into the facet accumulators."""
         off0, off1 = subgrid_config.off0, subgrid_config.off1
         subgrid = _to_device(_resolve(new_subgrid_task), self.device)
-        if self._fused:
+        if self._split:
+            done = self._add_subgrid_split(subgrid, off0, off1)
+        elif self._fused:
             done = self._add_subgrid_fused(subgrid, off0, off1)
         else:
             pieces = prepare_and_split_subgrid(
@@ -528,6 +541,64 @@ class SwiftlyBackward:
         self.task_queue.process(done)
         return done
 
+    def _column_for(self, off0):
+        """Column accumulators of subgrid column ``off0`` (LRU).  When a column has to make
+        room, it is folded into the facets first and its buffers are recycled."""
+        column = self.lru.get(off0)
+        if column is not None:
+            return column
+        reuse = None
+        if len(self.lru.data) >= self.lru.size:
+            # fold the column that is about to be evicted NOW and recycle its buffers:
+            # allocating the new column first would hold two columns (2 x 16 GiB at N=65536)
+            # next to the 128 GiB of facet accumulators
+            old_off0, reuse = self.lru.data.popitem(last=False)
+            self.update_MNAF_BMNAFs(old_off0, reuse)
+        if reuse is not None:
+            column = reuse
+            for acc in column:
+                acc.zero_()
+        else:
+            shape = (self.core.xM_yN_size, self.core.yN_size)
+            column = [torch.zeros(shape, dtype=torch.complex128, device=self.device)
+                      for _ in self.facets_config_list]
+        self.lru.set(off0, column)
+        return column
+
+    def _add_subgrid_split(self, subgrid, off0, off1):
+        # K4T: the subgrid along axis 0 into one (m, xA) strip per distinct facet off0, kept
+        # C-ordered so that the axis-0 lines (columns) are adjacent in memory
+        shape = (len(self._rows), self.core.xM_yN_size, subgrid.shape[1])
+        if self._strips is None or tuple(self._strips.shape) != shape:
+            self._strips = torch.empty(shape, dtype=torch.complex128, device=self.device)
+        strips = self._strips
+        self.core.split_subgrid_axis(
+            [subgrid], 0, [off0], [[(strips[r], row) for r, (row, _) in enumerate(self._rows)]],
+            "store")
+        return self.add_strips(off0, [(strips[r], row, off1)
+                                      for r, (row, _) in enumerate(self._rows)])
+
+    def add_strips(self, off0, strips):
+        """K3T: add facet-row strips of subgrids of column ``off0`` to the facets' column
+        accumulators, ONE launch (per 16 strips / 64 facets) for all of them, in order.
+
+        :param strips: list of ``(strip, row_off0, subgrid_off1)``: an ``(m, subgrid size)``
+            device tensor, the facet ``off0`` it was cut for (K4T) and the subgrid's ``off1``;
+            strips of rows without a facet here are skipped
+        """
+        column = self._column_for(off0)
+        groups, offs, targets = [], [], []
+        for strip, row, off1 in strips:
+            members = self._row_members.get(row)
+            if not members:
+                continue
+            groups.append(strip)
+            offs.append(off1)
+            targets.append([(column[j], self.facets_config_list[j].off1) for j in members])
+        if groups:
+            self.core.split_subgrid_axis(groups, 1, offs, targets, "add")
+        return [DeviceTask(column[-1])] if column else []
+
     def _add_subgrid_fused(self, subgrid, off0, off1):
         core = self.core
         prepared = core.prepare_subgrid(subgrid, (off0, off1))
@@ -535,31 +606,11 @@ class SwiftlyBackward:
         for cfg in self.facets_config_list:
             if cfg.off0 not in blocks:
                 blocks[cfg.off0] = core.extract_from_subgrid(prepared, cfg.off0, axis=0)
-        column = self.lru.get(off0)
-        if column is None:
-            reuse = None
-            if len(self.lru.data) >= self.lru.size:
-                # fold the column that is about to be evicted NOW and recycle its buffers:
-                # allocating the new column first would hold two columns (2 x 16 GiB at
-                # N=65536) next to the 128 GiB of facet accumulators
-                old_off0, reuse = self.lru.data.popitem(last=False)
-                self.update_MNAF_BMNAFs(old_off0, reuse)
-            if reuse is not None:
-                column = reuse
-                for acc in column:
-                    acc.zero_()
-            else:
-                shape = (core.xM_yN_size, core.yN_size)
-                column = [torch.zeros(shape, dtype=torch.complex128, device=self.device)
-                          for _ in self.facets_config_list]
+        column = self._column_for(off0)
         core.subgrid_to_facets(
             [blocks[cfg.off0] for cfg in self.facets_config_list], column,
             [cfg.off1 for cfg in self.facets_config_list], off1)
-        tasks = [DeviceTask(column[-1])] if column else []
-        old_off0, old_column = self.lru.set(off0, column)
-        if old_off0 is not None:
-            self.update_MNAF_BMNAFs(old_off0, old_column)
-        return tasks
+        return [DeviceTask(column[-1])] if column else []
 
     def update_off0_NAF_MNAFs(self, off0, off1, new_NAF_NAF_tasks):
         """Accumulate along axis 1 into the column accumulators of column ``off0``."""

@@ -21,6 +21,7 @@ from .api import (
     make_full_subgrid_cover,
 )
 from .api_helper import make_facet_device
+from .core import split_launches
 from .distributed import SwiftlyBackwardSharded, SwiftlyForwardSharded, partition_facets
 from .fourier_algorithm import make_subgrid_from_sources
 
@@ -376,10 +377,12 @@ class BackwardBenchRunner:
     """Synthetic full-cover BACKWARD transform (subgrid -> facet, reference ``api.py:327-463``)
     of one parameter set: every subgrid of the cover is folded into every facet.
 
-    One step = ``add_new_subgrid_task`` for all subgrids in cover order (prepare_subgrid,
-    extract_from_subgrid(axis 0) per facet row, the fused subgrid_to_facets kernel, the fused
+    One step = ``add_new_subgrid_task`` for all subgrids in cover order (per subgrid the split
+    kernels K4T -- prepare_subgrid + extract_from_subgrid along axis 0 into one strip per facet
+    row -- and K3T -- the same along axis 1, added to the facets' column accumulators; the fused
     fold_column kernel whenever a subgrid column is complete) + ``finish()`` (finish_facet
-    along axis 0 for every facet).  The subgrid values do not influence the timing: ``n_inputs``
+    along axis 0 for every facet).  Plans without the split kernel run prepare_subgrid,
+    extract_from_subgrid(axis 0) per facet row and subgrid_to_facets instead.  The subgrid values do not influence the timing: ``n_inputs``
     distinct random subgrids (2 GiB at N=65536, far larger than L2) are fed cyclically, which
     keeps the memory a full set would need free for the facet accumulators (2 GiB per facet at
     N=65536).  ``facet_offsets`` selects a sparse cover as in :class:`ForwardBenchRunner`.
@@ -514,8 +517,10 @@ class BackwardBenchRunner:
                            "facet; max|got - truth| / max|truth|"}
 
     def kernel_rooflines(self, hbm_gbs):
-        """CUDA-event timings of the fused backward kernels in the shapes the step launches,
-        with their algorithmic bytes (compulsory reads + read-modify-write of the accumulators)."""
+        """CUDA-event timings of the backward kernels in the shapes the step launches (K4T,
+        K3T, fold_column, finish_facet; the primitive subgrid side for plans without the split
+        kernel), with their algorithmic bytes (compulsory reads + writes, read-modify-write of the
+        accumulators)."""
         core, dev = self.core, self.device
         p = self.params
         yB, yN, xA, xM = p["yB_size"], p["yN_size"], p["xA_size"], p["xM_size"]
@@ -542,18 +547,52 @@ class BackwardBenchRunner:
 
         out = {}
         x = self.inputs[0]
-        t = timeit(lambda: core.prepare_subgrid(x, (sg.off0, sg.off1)))
-        out["prepare_subgrid (both axes)"] = (t, 16.0 * (xA * xA + 2 * xM * xA + xM * xM), S)
-        prepared = core.prepare_subgrid(x, (sg.off0, sg.off1))
-        t = timeit(lambda: [core.extract_from_subgrid(prepared, o, axis=0) for o in rows])
-        out["extract_from_subgrid axis 0 (all local facet rows)"] = (
-            t, 16.0 * len(rows) * (m * xM + m * xM), S)
-        blocks = {o: core.extract_from_subgrid(prepared, o, axis=0) for o in rows}
         accs = [torch.zeros((m, yN), dtype=torch.complex128, device=dev) for _ in local]
-        t = timeit(lambda: core.subgrid_to_facets(
-            [blocks[fcs[i].off0] for i in local], accs, [fcs[i].off1 for i in local], sg.off1))
-        out["subgrid_to_facets (extract axis 1 + accumulate, all local facets)"] = (
-            t, 16.0 * F * 3 * m * m, S)
+        if core.split_axis_supported():
+            # K4T: the supplier's subgrid into strips for every rank's facet rows (one call per
+            # supplied subgrid); K3T: the strips of a run of subgrids of one subgrid column in a
+            # batch of `world` into the local facets' column accumulators (one call per run).
+            # Calls per step are counted from the cover in step order; a call is one or more
+            # launches (split_launches).  K3T is timed for a full batch of `world` subgrids: at
+            # world > 1 the shorter runs at subgrid-column boundaries cost less than that.
+            all_rows = [sorted({fcs[i].off0 for i, o in enumerate(owner) if o == r})
+                        for r in range(self.world)]
+            n_strips = sum(len(r) for r in all_rows)
+            strips = torch.empty((max(1, n_strips), m, xA), dtype=torch.complex128, device=dev)
+            targets = [(strips[k], o) for k, o in enumerate(o for r in all_rows for o in r)]
+            k4_calls = len(range(self.rank, S, self.world))
+            t = timeit(lambda: core.split_subgrid_axis([x], 0, [sg.off0], [targets], "store"))
+            out[f"K4T split_subgrid_axis axis 0 ({n_strips} facet-row strips; per call, "
+                f"{split_launches([n_strips])} launch(es))"] = (
+                t, 16.0 * (xA * xA + n_strips * m * xA), k4_calls)
+            members = {o: [(accs[j], fcs[i].off1) for j, i in enumerate(local)
+                           if fcs[i].off0 == o] for o in rows}
+            groups = [(strips[k % len(strips)], o) for _ in range(self.world)
+                      for k, o in enumerate(rows)]
+            k3_calls = 0
+            for lo in range(0, S, self.world):
+                batch = self.sg_cfgs[lo:lo + self.world]
+                k3_calls += 1 + sum(1 for a, b in zip(batch, batch[1:]) if a.off0 != b.off0)
+            per_row = [len(members[o]) for o in rows]
+            t = timeit(lambda: core.split_subgrid_axis(
+                [g for g, _ in groups], 1, [sg.off1] * len(groups),
+                [members[o] for _, o in groups], "add"))
+            out[f"K3T split_subgrid_axis axis 1 ({self.world} subgrid(s) x {len(rows)} local "
+                f"facet rows, add to {F} facets; per call, "
+                f"{split_launches(per_row * self.world)} launch(es))"] = (
+                t, 16.0 * self.world * (len(rows) * m * xA + 2 * F * m * m), k3_calls)
+        else:
+            t = timeit(lambda: core.prepare_subgrid(x, (sg.off0, sg.off1)))
+            out["prepare_subgrid (both axes)"] = (t, 16.0 * (xA * xA + 2 * xM * xA + xM * xM), S)
+            prepared = core.prepare_subgrid(x, (sg.off0, sg.off1))
+            t = timeit(lambda: [core.extract_from_subgrid(prepared, o, axis=0) for o in rows])
+            out["extract_from_subgrid axis 0 (all local facet rows)"] = (
+                t, 16.0 * len(rows) * (m * xM + m * xM), S)
+            blocks = {o: core.extract_from_subgrid(prepared, o, axis=0) for o in rows}
+            t = timeit(lambda: core.subgrid_to_facets(
+                [blocks[fcs[i].off0] for i in local], accs, [fcs[i].off1 for i in local], sg.off1))
+            out["subgrid_to_facets (extract axis 1 + accumulate, all local facets)"] = (
+                t, 16.0 * F * 3 * m * m, S)
         faccs = [torch.zeros((yN, fcs[i].size), dtype=torch.complex128, device=dev)
                  for i in local[:8]]
         n8 = len(faccs)

@@ -34,6 +34,20 @@ def _is_tensor(a):
     return torch is not None and isinstance(a, torch.Tensor)
 
 
+def split_launches(group_sizes, max_groups=16, max_targets=64):
+    """Kernel launches of one ``split_subgrid_axis`` call with these targets per group: the
+    library cuts a group into pieces of at most 64 targets and packs pieces in order into
+    launches of at most 16 pieces and 64 targets (capi_backward.cu)."""
+    pieces = [min(max_targets, n - k) for n in group_sizes if n > 0
+              for k in range(0, n, max_targets)]
+    launches, groups, used = 0, 0, 0
+    for p in pieces:
+        if launches == 0 or groups == max_groups or used + p > max_targets:
+            launches, groups, used = launches + 1, 0, 0
+        groups, used = groups + 1, used + p
+    return launches
+
+
 class PreparedSumFinish:
     """Reusable argument block of a grouped ``sum_finish_axis`` launch (see
     :meth:`SwiftlyCoreB200.prepare_sum_finish`)."""
@@ -658,6 +672,61 @@ class SwiftlyCoreB200:
         _lib.check(self._lib, rc)
 
     # ------------------------------------------------------------------ fused backward path
+    def split_axis_supported(self):
+        """True if the fused subgrid split kernel exists for this (xM_yN_size, xM_size) pair."""
+        return self._lib.swiftly_b200_split_axis_supported(self._plan) > 0
+
+    def split_subgrid_axis(self, groups, axis, subgrid_offs, targets, mode):
+        """The subgrid side of the backward transform along ``axis``, ONE kernel per call.
+
+        Per line of ``groups[g]``: ``prepare_subgrid`` along ``axis`` with ``subgrid_offs[g]``
+        (core.py:328-368), then ``extract_from_subgrid(., facet_off, axis)`` (core.py:370-406)
+        for every target of the group; the adjoint of :meth:`sum_finish_axis`.
+
+        :param groups: 2-D complex128 device tensors, one per group; ``axis`` has the subgrid
+            size, the other axis the same line count in every group
+        :param subgrid_offs: one subgrid offset (along ``axis``) per group
+        :param targets: per group a list of ``(tensor, facet_off)``; the tensors have the
+            group's line count along the other axis and, along ``axis``,
+            ``xM_yN_size`` samples (``mode="store"``: overwritten with the contribution) or
+            ``yN_size`` samples (``mode="add"``: ``add_to_facet(., subgrid_off, axis)``,
+            core.py:408-449, accumulates into it).  In add mode the targets of one group must be
+            distinct tensors; different groups may share one (they are applied in order).
+        """
+        if axis not in (0, 1):
+            raise ValueError(f"Invalid axis {axis}")
+        if mode not in ("store", "add"):
+            raise ValueError(f"mode must be 'store' or 'add', not {mode!r}")
+        if len(subgrid_offs) != len(groups) or len(targets) != len(groups):
+            raise ValueError("subgrid_offs / targets must have one entry per group")
+        if not groups:
+            return targets
+        other = 1 - axis
+        size = self.yN_size if mode == "add" else self.xM_yN_size
+        ins = (_lib.Lines * len(groups))()
+        for g, t in enumerate(groups):
+            self._check_tensor(t)
+            if t.dtype != torch.complex128 or t.dim() != 2:
+                raise ValueError("subgrid inputs must be 2-D complex128 device tensors")
+            ins[g] = self._describe(t, axis)
+        flat = [tg for grp in targets for tg in grp]
+        arr = (_lib.SplitTarget * max(1, len(flat)))()
+        for i, (t, facet_off) in enumerate(flat):
+            self._check_tensor(t)
+            if t.dtype != torch.complex128 or t.dim() != 2:
+                raise ValueError("targets must be 2-D complex128 device tensors")
+            if t.shape[axis] != size:
+                raise ValueError(f"target has {t.shape[axis]} samples per line, expected {size}")
+            arr[i] = _lib.SplitTarget(t.data_ptr(), t.shape[other], t.stride(other),
+                                      t.stride(axis), int(facet_off))
+        sizes = (ctypes.c_int32 * len(groups))(*[len(grp) for grp in targets])
+        offs = (ctypes.c_int64 * len(groups))(*[int(o) for o in subgrid_offs])
+        rc = self._lib.swiftly_b200_split_subgrid_axis(
+            self._plan, ins, len(groups), offs, arr, sizes,
+            _lib.SPLIT_ADD if mode == "add" else _lib.SPLIT_STORE, self._stream(groups[0]))
+        _lib.check(self._lib, rc)
+        return targets
+
     def _lines_array(self, tensors, shape_check):
         arr = (_lib.Lines * len(tensors))()
         for k, t in enumerate(tensors):

@@ -507,6 +507,21 @@ SW_HD void line_fft_mixed(int lt, double* sm, const cplx* tw, Ld& ld, St& st, Sy
     }
 }
 
+// Number of sync() calls one line_fft_any<N> makes (plain barrier, no phase hooks): 4 per
+// Stockham pass after the first radix-16 pass, less one (the last pass stores straight from
+// registers), plus one for the combine of a mixed-radix line.  Threads that skip a transform
+// whose barrier is CTA-wide call sync() this many times instead (SubgridSplitAxisKernel).
+constexpr int ilog2_floor(int n) { return n <= 1 ? 0 : 1 + ilog2_floor(n / 2); }
+template <int N, bool POW2 = (N & (N - 1)) == 0>
+struct LineBarriers {
+    static constexpr int PASSES = (ilog2_floor(N) + 3) / 4 - 1;  // Stockham passes after the first
+    static constexpr int V = PASSES > 0 ? 4 * PASSES - 1 : 0;
+};
+template <int N>
+struct LineBarriers<N, false> {
+    static constexpr int V = LineBarriers<LineCfg<N>::P>::V + 1;
+};
+
 // line_fft for every length the fused subgrid kernels take: the Stockham plan for powers of
 // two, the mixed-radix line otherwise (work area: LineCfg<N>::SCRATCH doubles)
 template <int N, int DIR, class Ld, class St, class Sync>

@@ -797,4 +797,148 @@ struct SubgridAxisKernel {
     }
 };
 
+// ------------------------------------------------------------------ fused subgrid split kernel
+// The adjoint of SubgridAxisKernel: one axis of "prepare a subgrid and cut it into the
+// contributions of several facets":
+//   for every input line l:
+//     acc[0..xM) = fft_c(roll(pad_mid(in[l], xM), off))      (prepare_subgrid, core.py:328-368)
+//     for every target j:  w[(u + sf_j) mod m] = Fn[u] * acc[(xM/2 - m/2 + u + sf_j) mod xM]
+//                          c = ifft_c(w)                      (extract_from_subgrid, core.py:370-406)
+//       store mode:  out_j[l, t] = c[t]
+//       add mode:    out_j[l, (yN/2 - m/2 + s + ((t - s) mod m)) mod yN] += c[t],  s = off yN / N
+//                                                           (add_to_facet, core.py:408-449)
+// The prepared xM-point line lives in shared memory only.  The targets only READ it, so their
+// windows may overlap or repeat: targets are processed CONC = xM/m at a time in the order given,
+// and a round with fewer targets leaves its idle transform slots idle (no transform of zeros).
+// A CTA takes a line (two adjacent lines with LINES = 2) and runs it through EVERY group of the
+// launch in order, so every (target, line) is written by exactly one CTA even when targets of
+// different groups share an accumulator (a batch of subgrids of one subgrid column): no
+// atomics, and the sums are formed in group order.
+struct SplitTarget {
+    cplx* base;          // line 0, sample 0 of the target
+    int64_t ls, es;      // line / sample stride (complex elements)
+    int sf_m, pos_base;  // facet_off * xM // N mod m ; (xM/2 - m/2 + sf) mod xM
+};
+struct SplitGroup {
+    const cplx* in;     // input lines (sz samples each)
+    int64_t in_ls, in_es;
+    int sz, start;      // subgrid size ; (xM/2 - sz//2 + subgrid_off) mod xM
+    int s_m, base_y;    // add mode: subgrid_off * yN // N mod m ; (yN/2 - m/2 + s) mod yN
+    int first, count;   // targets [first, first + count) of the launch's table
+};
+
+// CTA barrier that the threads of one warp may reach from DIFFERENT places in the code
+// (barrier.sync without .aligned; __syncthreads is the aligned form, which requires the whole
+// warp to execute the same barrier instruction)
+template <class Ctx>
+SW_HD void cta_sync_divergent(const Ctx& ctx) {
+#if defined(__CUDA_ARCH__) && !defined(SWIFTLY_EMU)
+    (void)ctx;
+    asm volatile("barrier.sync 0;" ::: "memory");
+#else
+    ctx.sync();
+#endif
+}
+
+template <int M, int XM, int LINES>
+struct SubgridSplitAxisKernel {
+    static constexpr int T_M = LineCfg<M>::T;
+    static constexpr int T_X = LineCfg<XM>::T;
+    static constexpr int THREADS = T_X * LINES;
+    static constexpr int CONC = T_X / T_M;
+    // shared memory layout as in SubgridAxisKernel
+    static constexpr int WSTRIDE = SubgridAxisKernel<M, XM, LINES>::WSTRIDE;
+    static constexpr int WORK = SubgridAxisKernel<M, XM, LINES>::WORK;
+    static constexpr int ACCS = SubgridAxisKernel<M, XM, LINES>::ACCS;
+    static constexpr size_t SMEM = SubgridAxisKernel<M, XM, LINES>::SMEM;
+    static constexpr bool WARP_BOUNDS = SubgridAxisKernel<M, XM, LINES>::WARP_BOUNDS;
+    // transforms of whole warps synchronise on a named barrier of their own; otherwise the
+    // barrier is CTA-wide and the threads of an idle slot take part in it -- from another place
+    // in the code than the transform's threads of the same warp, hence the non-aligned barrier
+    static constexpr bool GROUP_BARRIERS = (T_M * LINES) % 32 == 0 && CONC > 1 && CONC <= 15;
+
+    SplitTarget tgt[SW_MAX_SOURCES];
+    SplitGroup grp[SW_MAX_GROUPS];
+    int n_groups;
+    int64_t n_lines;  // every group
+    int add;          // 0: store mode, 1: add-to-facet mode
+    int yN;
+    const double* fn;
+    const cplx* tw_m;
+    const cplx* tw_x;
+    double scale;  // 1 / m
+
+    template <class Ctx>
+    SW_HD void operator()(Ctx& ctx) const {
+        const int sub = ctx.tid % LINES;
+        const int t = ctx.tid / LINES;
+        cplx* acc = (cplx*)ctx.smem + (size_t)sub * ACCS;
+        double* work = (double*)((cplx*)ctx.smem + (size_t)LINES * ACCS) + (size_t)sub * WORK;
+        const int c = t / T_M;
+        const int lt = t % T_M;
+        auto sync = [&]() { ctx.sync(); };
+        auto gsync = [&]() {
+            if (GROUP_BARRIERS)
+                ctx.group_sync(1 + c, T_M * LINES);
+            else
+                cta_sync_divergent(ctx);
+        };
+        const int64_t lines_cta = (n_lines + LINES - 1) / LINES;
+        for (int64_t wl = ctx.bid; wl < lines_cta; wl += ctx.nblocks) {
+            const int64_t line = wl * LINES + sub;
+            const bool line_ok = line < n_lines;
+            for (int g = 0; g < n_groups; ++g) {
+                const int count = grp[g].count;
+                if (count == 0) continue;
+                {
+                    const cplx* in = grp[g].in + (line_ok ? line : 0) * grp[g].in_ls;
+                    const int64_t in_es = grp[g].in_es;
+                    const int sz = grp[g].sz, start = grp[g].start;
+                    auto ld = [&](int q) {
+                        int r = wrap_sub(wrap_add(q, XM / 2, XM), start, XM);
+                        if (!line_ok || r >= sz) return mk(0.0, 0.0);
+                        return ld_stream(in + (int64_t)r * in_es);
+                    };
+                    auto st = [&](int p, cplx v) { acc[wrap_add(p, XM / 2, XM)] = v; };
+                    line_fft_any<XM, -1>(t, work, tw_x, ld, st, sync);
+                }
+                ctx.sync();  // acc complete; the work area is free for the m-point transforms
+                const int s_m = grp[g].s_m, base_y = grp[g].base_y;
+                for (int k0 = 0; k0 < count; k0 += CONC) {
+                    if (k0 + c < count) {
+                        const SplitTarget& T = tgt[grp[g].first + k0 + c];
+                        cplx* base = T.base + (line_ok ? line : 0) * T.ls;
+                        const int64_t es = T.es;
+                        const int sf_m = T.sf_m, pos_base = T.pos_base;
+                        auto ld = [&](int q) {
+                            int u = wrap_sub(wrap_add(q, M / 2, M), sf_m, M);
+                            return cscale(acc[wrap_add(pos_base, u, XM)], ldg_d(fn + u));
+                        };
+                        auto st = [&](int p, cplx v) {
+                            if (!line_ok) return;
+                            int pc = wrap_add(p, M / 2, M);
+                            if (add) {
+                                int w = wrap_add(base_y, wrap_sub(pc, s_m, M), yN);
+                                cplx* o = base + (int64_t)w * es;
+                                cplx a = *o;
+                                *o = mk(a.x + scale * v.x, a.y + scale * v.y);
+                            } else {
+                                st_stream(base + (int64_t)pc * es, cscale(v, scale));
+                            }
+                        };
+                        line_fft_any<M, +1>(lt, work + (size_t)c * WSTRIDE, tw_m, ld, st, gsync);
+                    } else if constexpr (!GROUP_BARRIERS) {
+                        for (int i = 0; i < LineBarriers<M>::V; ++i) cta_sync_divergent(ctx);
+                    }
+                    // work areas are reused by the next round / the next line
+                    if constexpr (GROUP_BARRIERS)
+                        ctx.sync();
+                    else
+                        cta_sync_divergent(ctx);
+                }
+            }
+        }
+    }
+};
+
 }  // namespace swiftly

@@ -91,4 +91,17 @@ bool make_row_map(TensorMap4* tm, const cplx* base, int64_t ls, int64_t n_rows, 
 int subgrid_axis_conc(int m, int xM);
 int run_subgrid_axis(const swiftly_b200* h, const SubgridAxisArgs& a, cudaStream_t s);
 
+// fused subgrid split kernel (dispatch_subgrid_split.cu), the backward direction's adjoint of
+// the above: groups share the line count; targets are [grp[g].first, + grp[g].count)
+struct SubgridSplitArgs {
+    SplitTarget tgt[SW_MAX_SOURCES];
+    SplitGroup grp[SW_MAX_GROUPS];
+    int n_groups;
+    int64_t n_lines;
+    int add;
+};
+// concurrent m-point transforms per line (xM / m, at least 1), 0 if the pair has no kernel
+int subgrid_split_conc(int m, int xM);
+int run_subgrid_split(const swiftly_b200* h, const SubgridSplitArgs& a, cudaStream_t s);
+
 }  // namespace swiftly

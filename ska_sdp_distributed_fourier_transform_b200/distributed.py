@@ -484,12 +484,18 @@ class SwiftlyBackwardSharded:
     """Subgrid -> facet accumulation with the facets sharded over a process group.
 
     Mirror image of :class:`SwiftlyForwardSharded` (SURVEY.md section 8e): every facet
-    accumulator lives on the rank that owns the facet (:func:`partition_facets`), so the only
-    exchange is getting each subgrid to every rank -- subgrids are processed in batches of
-    ``world_size``, subgrid ``b`` of a batch is supplied by rank ``b`` (the rank that owns it
-    after the forward transform) and one ``all_gather`` per batch replicates the batch; there
-    is no reduction.  Each rank then folds the batch into its own facets with the fused
-    backward kernels of :class:`~.api.SwiftlyBackward`.
+    accumulator lives on the rank that owns the facet (:func:`partition_facets`).  Subgrids are
+    processed in batches of ``world_size``; subgrid ``b`` of a batch is supplied by rank ``b``
+    (the rank that owns it after the forward transform).  That rank cuts it along axis 0 into
+    strips, one ``(m, xA)`` strip per facet row of EVERY rank (the split kernel K4T, written
+    straight into a ``(world, rows_max, m, xA)`` send buffer; a facet row split over two ranks
+    is cut for both), one ``all_to_all`` per batch moves the strips to the facets' owners, and
+    each rank adds the strips of the whole batch to its facets' column accumulators (K3T, one
+    launch per run of subgrids of the same subgrid column, in subgrid order).  Per batch a rank
+    receives ``world * rows_max * m * xA`` samples -- its own facet rows only -- and the subgrid
+    side is computed once per subgrid, not once per rank.  Plans without the split kernel
+    replicate every subgrid with one ``all_gather`` per batch instead and run the fused
+    backward kernels of :class:`~.api.SwiftlyBackward` on every rank.
 
     Calls are collective: every rank calls :meth:`add_subgrid_tasks` with the same subgrid
     configs; ``tasks[i]`` must be given on rank ``i % world_size`` (others pass ``None``).
@@ -510,6 +516,66 @@ class SwiftlyBackwardSharded:
         self._local = SwiftlyBackward(
             swiftly_config, [self.facets_config_list[i] for i in self.local_idx],
             lru_backward=lru_backward, queue_size=queue_size)
+        self.core = swiftly_config.core
+        # strip layout as in SwiftlyForwardSharded: per rank the sorted distinct off0 of its facets
+        self.rank_rows = []
+        for r in range(self.world):
+            self.rank_rows.append(sorted({self.facets_config_list[i].off0
+                                          for i, o in enumerate(self.owner) if o == r}))
+        self.rows_max = max(1, max(len(r) for r in self.rank_rows))
+        self.my_rows = self.rank_rows[self.rank]
+        self._split = self._local._split
+        self._bufs = {}
+
+    def _strip_buffers(self, xA):
+        """(send, recv) of shape ``(world, rows_max, m, xA)``; strip ``[r, k]`` is the strip of
+        facet row ``rank_rows[r][k]``, C-ordered (the axis-0 lines of K4T are adjacent)."""
+        if xA not in self._bufs:
+            shape = (self.world, self.rows_max, self.core.xM_yN_size, xA)
+            self._bufs[xA] = (torch.zeros(shape, dtype=torch.complex128, device=self.device),
+                              torch.zeros(shape, dtype=torch.complex128, device=self.device))
+        return self._bufs[xA]
+
+    def _supplied(self, tasks, mine, xA):
+        from .api import _resolve, _to_device  # pylint: disable=import-outside-toplevel
+
+        data = tasks[mine]
+        if data is None:
+            raise ValueError(f"rank {self.rank} must supply subgrid {mine}")
+        sub = _to_device(_resolve(data), self.device)
+        if tuple(sub.shape) != (xA, xA):
+            raise ValueError(f"subgrid {mine} has shape {tuple(sub.shape)}, expected {(xA, xA)}")
+        return sub
+
+    def _add_batch_split(self, batch, lo, tasks):
+        """One batch on the split kernels: K4T of my subgrid into the send buffer, all_to_all,
+        K3T of the received strips into my facets' column accumulators."""
+        xA = batch[0].size
+        send, recv = self._strip_buffers(xA)
+        if self.rank < len(batch):
+            sub = self._supplied(tasks, lo + self.rank, xA)
+            sg = batch[self.rank]
+            targets = [(send[r, k], off0) for r in range(self.world)
+                       for k, off0 in enumerate(self.rank_rows[r])]
+            self.core.split_subgrid_axis([sub], 0, [sg.off0], [targets], "store")
+        if self.world > 1:
+            dist.all_to_all_single(torch.view_as_real(recv).view(self.world, -1),
+                                   torch.view_as_real(send).view(self.world, -1),
+                                   group=self.group)
+        else:
+            recv = send
+        if not self.my_rows:
+            return
+        b = 0
+        while b < len(batch):  # runs of consecutive subgrids of the same subgrid column
+            e = b + 1
+            while e < len(batch) and batch[e].off0 == batch[b].off0:
+                e += 1
+            done = self._local.add_strips(batch[b].off0, [
+                (recv[s, k], off0, batch[s].off1)
+                for s in range(b, e) for k, off0 in enumerate(self.my_rows)])
+            self._local.task_queue.process(done)  # queue_size bounds the results in flight
+            b = e
 
     def add_subgrid_tasks(self, subgrid_configs, tasks):
         """Fold ``subgrid_configs`` into the local facets (collective call)."""
@@ -522,6 +588,9 @@ class SwiftlyBackwardSharded:
             raise ValueError("all subgrids of one call must have the same size")
         for lo in range(0, len(subgrid_configs), self.world):
             batch = subgrid_configs[lo:lo + self.world]
+            if self._split:
+                self._add_batch_split(batch, lo, tasks)
+                continue
             mine = lo + self.rank
             xA = batch[0].size
             if self.rank < len(batch):
