@@ -43,6 +43,7 @@ int launch_split(const swiftly_b200* h, const Op& op, cudaStream_t s) {
     if (!tw || !tw2) return SWIFTLY_B200_ECUDA;
     // persistent CTAs: two per SM's worth of lines in flight keeps the scratch L2 resident
     int64_t blocks = op.g.n_lines < 296 ? op.g.n_lines : 296;
+    if (h->max_blocks > 0 && blocks > h->max_blocks) blocks = h->max_blocks;  // (test hook)
     cplx* scratch = split_scratch(h, s, (size_t)blocks * H);
     if (!scratch) return SWIFTLY_B200_ECUDA;
     SplitLineKernel<H, DIR, Op> k{op, tw, tw2, scratch};
@@ -57,6 +58,7 @@ int launch_split_f(const swiftly_b200* h, const Op& op, int F, cudaStream_t s) {
     const cplx* twf = twiddles_full(h, (int)n);
     if (!tw || !twf) return SWIFTLY_B200_ECUDA;
     int64_t blocks = op.g.n_lines < 296 ? op.g.n_lines : 296;
+    if (h->max_blocks > 0 && blocks > h->max_blocks) blocks = h->max_blocks;  // (test hook)
     cplx* scratch = split_scratch(h, s, (size_t)blocks * (size_t)(F - 1) * M);
     if (!scratch) return SWIFTLY_B200_ECUDA;
     SplitFKernel<M, DIR, Op> k;
