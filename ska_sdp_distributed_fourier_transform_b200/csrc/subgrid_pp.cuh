@@ -290,6 +290,14 @@ struct SubgridAxisKernelPP {
                         for (int i = t; i < XM; i += T_X) acc[i] = mk(0.0, 0.0);
                     continue;
                 }
+                // The transform's per-thread shared-memory offsets and twiddle addresses depend
+                // on lt alone.  Left visible, the compiler computes them once per kernel and
+                // keeps them live across every line, which overflows the 128-register budget and
+                // spills them (plus transform data) to local memory, reloaded inside each pass
+                // through an L1 the 209 KiB carveout has shrunk to ~28 KB.  An opaque copy of lt
+                // per round makes them a few integer instructions per pass instead.
+                int lt_r = lt;
+                asm volatile("" : "+r"(lt_r));
                 const bool cx = overwrite && cx_round0 && (!skip_empty || act == (1u << CONC) - 1);
                 if (tma_wait_due && !cx) {
                     msync.tma_pending = true;
@@ -325,10 +333,10 @@ struct SubgridAxisKernelPP {
                     // the accumulator then have to wait until every transform of the round has
                     // left its buffer: the pre-store group barrier.
                     msync.order_stores = true;
-                    line_fft_cx<M, -1, false>(lt, acc + (size_t)c * (M + M / 16), tw_m, ld, st, msync);
+                    line_fft_cx<M, -1, false>(lt_r, acc + (size_t)c * (M + M / 16), tw_m, ld, st, msync);
                 } else {
                     msync.order_stores = slot0 > 0;
-                    line_fft<M, -1>(lt, work + (size_t)c * WSTRIDE, tw_m, ld, st, msync);
+                    line_fft<M, -1>(lt_r, work + (size_t)c * WSTRIDE, tw_m, ld, st, msync);
                 }
             }
             if (tma_wait_due && t == 0) ctx.bulk_wait_read();  // (no round used the work area)
@@ -356,8 +364,10 @@ struct SubgridAxisKernelPP {
                     }
                 };
                 // the exchange buffer IS the accumulator: the acquire() (a group barrier) of
-                // the first pass comes after every thread's loads
-                line_fft_cx<XM, +1, true>(t, acc, tw_x, ld, st, gsync);
+                // the first pass comes after every thread's loads; t_r: as lt_r above
+                int t_r = t;
+                asm volatile("" : "+r"(t_r));
+                line_fft_cx<XM, +1, true>(t_r, acc, tw_x, ld, st, gsync);
             }
             gsync();  // accumulator is rewritten by the next line; staged line complete
             if (tma_out && t == 0 && line_ok) {
