@@ -144,6 +144,7 @@ extern "C" int swiftly_b200_create(double W, int64_t N, int64_t xM, int64_t yN, 
     h->force_split = 0;
     h->sg_variant = 0;
     h->max_blocks = 0;
+    for (int i = 0; i < 4; ++i) h->last_launch[i] = 0;
     cudaError_t e = cudaMalloc((void**)&h->d_Fb, sizeof(double) * (size_t)(yN > 1 ? yN - 1 : 1));
     if (e == cudaSuccess) e = cudaMalloc((void**)&h->d_Fn, sizeof(double) * (size_t)h->m);
     if (e == cudaSuccess)
@@ -201,6 +202,16 @@ extern "C" void swiftly_b200_debug_max_blocks(swiftly_b200* h, int blocks) {
 
 extern "C" void swiftly_b200_debug_sg_variant(swiftly_b200* h, int variant) {
     if (h) h->sg_variant = variant;
+}
+
+// test hook (not in the public header): the form of the last fused subgrid launch, so that a
+// test can assert the kernel it was written for.  out[0]: kernel (0 none yet, 1 round-1
+// SubgridAxisKernel, 2 two-group SubgridAxisKernelPP, 3 split SubgridSplitAxisKernel);
+// out[1]: lines per CTA; out[2]: output path (0 direct stores, 1 TMA with one tensor map,
+// 2 TMA with one tensor map per group); out[3]: grid size
+extern "C" void swiftly_b200_debug_last_launch(const swiftly_b200* h, int* out) {
+    if (h && out)
+        for (int i = 0; i < 4; ++i) out[i] = h->last_launch[i];
 }
 
 // ------------------------------------------------------------------ host staging

@@ -30,6 +30,7 @@ static int launch_sg_axis_l(const swiftly_b200* h, const SubgridAxisArgs& a, cud
     k.accumulate_out = a.accumulate_out;
     int grid = grid_for(((a.n_lines + LINES - 1) / LINES) * a.n_groups, 1);
     if (h->max_blocks > 0 && grid > h->max_blocks) grid = h->max_blocks;  // (test hook)
+    note_launch(h, 1, LINES, 0, grid);
     cudaError_t e = launch_body(k, grid, k.SMEM, s);
     return e == cudaSuccess ? SWIFTLY_B200_OK : cuda_fail(e, "subgrid axis kernel launch");
 }
@@ -107,23 +108,23 @@ static int launch_sg_axis_pp(const swiftly_b200* h, const SubgridAxisArgs& a, cu
     // persistent: one CTA per SM, every CTA walks over line pairs
     int64_t pairs = ((a.n_lines + 1) / 2) * a.n_groups;
     int grid = (int)(pairs < NUM_SMS ? pairs : NUM_SMS);
+    if (h->max_blocks > 0 && grid > h->max_blocks) grid = h->max_blocks;  // (test hook)
+    note_launch(h, 2, 2, k.tma_out ? 1 + k.tma_per_group : 0, grid);
     cudaError_t e = launch_body_maps(k, maps, grid, k.SMEM, s);
     return e == cudaSuccess ? SWIFTLY_B200_OK : cuda_fail(e, "subgrid axis (two-group) kernel launch");
 }
 
 // The two-group kernel takes power-of-two lengths with CONC = 2 or 4.  The catalogue's other
 // pairs run the round-1 kernel: CONC = 8 (m = 128, xM = 1024: eight-thread transforms), CONC = 1
-// (m = xM = 256: one source per round) and the mixed-radix lengths (3, 5, 7 * 2^k).
+// (m = xM = 256: one source per round) and the mixed-radix lengths (3, 5, 7 * 2^k).  A thread
+// group must be whole warps (xM >= 512) and both groups must fit shared memory (xM <= 4096).
+// The emulated build dispatches the same way, so that it runs the forms the GPU runs.
 template <int M, int XM>
 struct PingPongFits {
     static constexpr bool POW2 = (M & (M - 1)) == 0 && (XM & (XM - 1)) == 0 && XM / M >= 2;
-#if defined(SWIFTLY_EMU)
-    static constexpr bool V = POW2 && (XM / M) <= 4;
-#else
     static constexpr bool V = POW2 && (XM / M) <= 4 && (XM / 16) % 32 == 0 &&
                               2 * ((size_t)(XM + XM / 16) * 16 + (size_t)(XM + XM / 16 + 24) * 8) <=
                                   227 * 1024;
-#endif
 };
 
 // two adjacent lines per CTA when every source and the output have unit line stride

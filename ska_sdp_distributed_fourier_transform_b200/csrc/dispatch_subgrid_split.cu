@@ -19,6 +19,7 @@ static int launch_split_pair_l(const swiftly_b200* h, const SubgridSplitArgs& a,
     k.scale = 1.0 / (double)M;
     int grid = grid_for((a.n_lines + LINES - 1) / LINES, 1);
     if (h->max_blocks > 0 && grid > h->max_blocks) grid = h->max_blocks;  // (test hook)
+    note_launch(h, 3, LINES, 0, grid);
     cudaError_t e = launch_body(k, grid, k.SMEM, s);
     return e == cudaSuccess ? SWIFTLY_B200_OK : cuda_fail(e, "subgrid split kernel launch");
 }

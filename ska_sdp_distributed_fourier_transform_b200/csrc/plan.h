@@ -24,6 +24,9 @@ struct swiftly_b200 {
     int sg_variant;   // debug / test: fused subgrid kernel variant (dispatch_subgrid_axis.cu)
     int max_blocks;   // debug / test: cap of the persistent kernels' grid (0: none), so that a
                       // small test problem walks several lines per CTA
+    // debug / test: what the last fused subgrid launch ran (kernel, lines per CTA, output
+    // path, grid), see swiftly_b200_debug_last_launch
+    mutable int last_launch[4];
 };
 
 namespace swiftly {
@@ -37,6 +40,14 @@ const cplx* twiddles(const swiftly_b200* h, int n);
 const cplx* twiddles_full(const swiftly_b200* h, int n);
 // per-stream scratch of at least `samples` complex samples (grown on demand)
 cplx* split_scratch(const swiftly_b200* h, cudaStream_t s, size_t samples);
+
+// records the form of a fused subgrid launch for swiftly_b200_debug_last_launch
+inline void note_launch(const swiftly_b200* h, int kernel, int lines, int out_path, int grid) {
+    h->last_launch[0] = kernel;
+    h->last_launch[1] = lines;
+    h->last_launch[2] = out_path;
+    h->last_launch[3] = grid;
+}
 
 // SMs of the H100 SXM: grid size of the persistent kernels and cap of the grid-stride ones
 static const int NUM_SMS = 132;

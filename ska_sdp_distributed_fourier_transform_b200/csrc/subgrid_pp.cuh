@@ -44,9 +44,7 @@ struct SubgridAxisKernelPP {
     static constexpr int ACCS = XM + XM / 16;  // cplx per group: accumulator / xM exchange
     static constexpr size_t SMEM =
         (size_t)GROUPS * ((size_t)ACCS * sizeof(cplx) + (size_t)WORK * sizeof(double));
-#if !defined(SWIFTLY_EMU)
     static_assert(T_X % 32 == 0, "a thread group must be whole warps");
-#endif
     // named barriers need whole warps; smaller transforms use the group barrier
     static constexpr bool SUB_BARRIERS = (T_M % 32 == 0) && CONC > 1;
     // a slot without a source can sit its round out only when its transform's barriers are its

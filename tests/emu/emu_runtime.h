@@ -84,7 +84,8 @@ struct HostCtx {
     // named barriers with the hardware's counting semantics (bar.sync / bar.arrive a, b):
     // the barrier completes when `count` threads have arrived; bar.sync waits for that,
     // bar.arrive does not.  A protocol error (unbalanced arrivals) shows up as a deadlock,
-    // which the scheduler detects and reports instead of hanging.
+    // which the scheduler detects and reports instead of hanging; an id above 15 or a count
+    // that is not whole warps on a named barrier is reported as soon as it is used.
     inline void group_sync(int id, int count) const;
     inline void group_arrive(int id, int count) const;
     inline void yield() const;
@@ -147,8 +148,24 @@ inline void HostCtx::yield() const {
     swapcontext(&b->ctxs[tid], &b->main_ctx);
 }
 
+// bar.sync / bar.arrive take ids 0..15, and a thread count that is a multiple of the warp size
+// (barrier 0 is __syncthreads, whose count is the whole CTA): anything else is invalid on the
+// hardware, so the emulator reports it as a protocol error, like a deadlock.  A CTA of less than
+// one warp cannot form a whole-warp barrier at all: it is a kernel form forced at a line length
+// far below the one it serves on the GPU (the split K2 forms at yN = 512: 16-thread CTAs, whole
+// warps at yN = 16384), and only the id range is checked there.
+static inline void emu_check_barrier(int id, int count, int cta_threads) {
+    const bool warps = count > 0 && (count % 32 == 0 || cta_threads < 32);
+    if (id < 0 || id >= 16 || (id != 0 && !warps)) {
+        fprintf(stderr, "swiftly emulator: barrier PROTOCOL error (id %d, count %d): named barriers "
+                        "take ids 0..15 and whole warps\n", id, count);
+        abort();
+    }
+}
+
 inline void HostCtx::group_arrive(int id, int count) const {
     EmuBlock* b = blk;
+    emu_check_barrier(id, count, b->nthreads);
     if (++b->bar_arrived[id] >= count) {
         b->bar_arrived[id] = 0;
         ++b->bar_gen[id];
