@@ -204,11 +204,14 @@ extern "C" void swiftly_b200_debug_sg_variant(swiftly_b200* h, int variant) {
     if (h) h->sg_variant = variant;
 }
 
-// test hook (not in the public header): the form of the last fused subgrid launch, so that a
-// test can assert the kernel it was written for.  out[0]: kernel (0 none yet, 1 round-1
-// SubgridAxisKernel, 2 two-group SubgridAxisKernelPP, 3 split SubgridSplitAxisKernel);
-// out[1]: lines per CTA; out[2]: output path (0 direct stores, 1 TMA with one tensor map,
-// 2 TMA with one tensor map per group); out[3]: grid size
+// test hook (not in the public header): the form of the last kernel launch of the plan, so that
+// a test can assert the kernel it was written for.  out[0]: kernel (0 none yet, 1 round-1
+// SubgridAxisKernel, 2 two-group SubgridAxisKernelPP, 3 split SubgridSplitAxisKernel,
+// 4 LineKernel, 5 SplitLineKernel, 6 SplitFKernel, 7 WindowCopyKernel); out[1]: lines per CTA
+// (1 .. 4), F (5, 6: 2 for SplitLineKernel) or 0 (7); out[2]: output path of the fused kernels
+// (0 direct stores, 1 TMA with one tensor map, 2 TMA with one tensor map per group), the
+// line-fastest flag of 4 and 7, 0 for 5 and 6; out[3]: grid size.  The TMA-staged and parked
+// extract_columns forms are not recorded.
 extern "C" void swiftly_b200_debug_last_launch(const swiftly_b200* h, int* out) {
     if (h && out)
         for (int i = 0; i < 4; ++i) out[i] = h->last_launch[i];
@@ -346,6 +349,16 @@ bool lines_adjacent(const Lines& g) {
     return g.n_lines > 1 && (g.in_ls == 1 || g.out_ls == 1) && g.in_es != 1;
 }
 
+// grid of WindowCopyKernel for `total` samples: one per thread up to 64 CTAs per SM, a
+// grid-stride loop beyond; capped by the plan's max_blocks (test hook)
+int window_copy_grid(const swiftly_b200* h, int64_t total) {
+    const int64_t per_cta = WindowCopyKernel<false>::THREADS;
+    int64_t grid = (total + per_cta - 1) / per_cta;
+    if (grid > NUM_SMS * 64) grid = NUM_SMS * 64;
+    if (h->max_blocks > 0 && grid > h->max_blocks) grid = h->max_blocks;
+    return (int)grid;
+}
+
 }  // namespace
 
 #define SW_PROLOGUE(what, in_size, out_size, copy_out)                          \
@@ -469,8 +482,8 @@ extern "C" int swiftly_b200_extract_from_facet(const swiftly_b200* h,
     k.s_m = (int)pmod(sc, m);
     k.base = (int)pmod(yN / 2 - m / 2 + sc, yN);
     k.line_fastest = lines_adjacent(g) ? 1 : 0;
-    int64_t total = g.n_lines * m;
-    int grid = (int)((total + 255) / 256 < NUM_SMS * 64 ? (total + 255) / 256 : NUM_SMS * 64);
+    const int grid = window_copy_grid(h, g.n_lines * m);
+    note_launch(h, LAUNCH_WINDOW_COPY, 0, k.line_fastest, grid);
     SW_CUDA(launch_body(k, grid, 0, s), "extract_from_facet launch");
     return stage_out(sout, s);
 }
@@ -559,8 +572,8 @@ extern "C" int swiftly_b200_add_to_facet(const swiftly_b200* h, const swiftly_b2
     k.s_m = (int)pmod(sc, m);
     k.base = (int)pmod(yN / 2 - m / 2 + sc, yN);
     k.line_fastest = lines_adjacent(g) ? 1 : 0;
-    int64_t total = g.n_lines * m;
-    int grid = (int)((total + 255) / 256 < NUM_SMS * 64 ? (total + 255) / 256 : NUM_SMS * 64);
+    const int grid = window_copy_grid(h, g.n_lines * m);
+    note_launch(h, LAUNCH_WINDOW_COPY, 0, k.line_fastest, grid);
     SW_CUDA(launch_body(k, grid, 0, s), "add_to_facet launch");
     return stage_out(sout, s);
 }

@@ -20,18 +20,27 @@ inline int grid_for(int64_t n_lines, int lpc) {
     return (int)(blocks < cap ? blocks : cap);
 }
 
+// grid_for, further capped by the plan's max_blocks (test hook)
+inline int grid_for(const swiftly_b200* h, int64_t n_lines, int lpc) {
+    int grid = grid_for(n_lines, lpc);
+    return h->max_blocks > 0 && grid > h->max_blocks ? h->max_blocks : grid;
+}
+
 template <int N, int DIR, class Op>
 int launch_lines(const swiftly_b200* h, const Op& op, bool line_fastest, cudaStream_t s) {
     const cplx* tw = twiddles(h, N);
     if (!tw) return SWIFTLY_B200_ECUDA;
     constexpr int LPC = LinesPerCta<N>::V;
+    const int grid = grid_for(h, op.g.n_lines, LPC);
     cudaError_t e;
     if (line_fastest && LPC > 1) {
+        note_launch(h, LAUNCH_LINE, LPC, 1, grid);
         LineKernel<N, DIR, LPC, true, Op> k{op, tw};
-        e = launch_body(k, grid_for(op.g.n_lines, LPC), k.SMEM, s);
+        e = launch_body(k, grid, k.SMEM, s);
     } else {
+        note_launch(h, LAUNCH_LINE, LPC, 0, grid);
         LineKernel<N, DIR, LPC, false, Op> k{op, tw};
-        e = launch_body(k, grid_for(op.g.n_lines, LPC), k.SMEM, s);
+        e = launch_body(k, grid, k.SMEM, s);
     }
     return e == cudaSuccess ? SWIFTLY_B200_OK : cuda_fail(e, "line FFT kernel launch");
 }
@@ -46,6 +55,7 @@ int launch_split(const swiftly_b200* h, const Op& op, cudaStream_t s) {
     if (h->max_blocks > 0 && blocks > h->max_blocks) blocks = h->max_blocks;  // (test hook)
     cplx* scratch = split_scratch(h, s, (size_t)blocks * H);
     if (!scratch) return SWIFTLY_B200_ECUDA;
+    note_launch(h, LAUNCH_SPLIT_LINE, 2, 0, (int)blocks);
     SplitLineKernel<H, DIR, Op> k{op, tw, tw2, scratch};
     cudaError_t e = launch_body(k, (int)blocks, k.SMEM, s);
     return e == cudaSuccess ? SWIFTLY_B200_OK : cuda_fail(e, "split line FFT kernel launch");
@@ -61,6 +71,7 @@ int launch_split_f(const swiftly_b200* h, const Op& op, int F, cudaStream_t s) {
     if (h->max_blocks > 0 && blocks > h->max_blocks) blocks = h->max_blocks;  // (test hook)
     cplx* scratch = split_scratch(h, s, (size_t)blocks * (size_t)(F - 1) * M);
     if (!scratch) return SWIFTLY_B200_ECUDA;
+    note_launch(h, LAUNCH_SPLIT_F, F, 0, (int)blocks);
     SplitFKernel<M, DIR, Op> k;
     k.op = op;
     k.tw = tw;

@@ -24,8 +24,9 @@ struct swiftly_b200 {
     int sg_variant;   // debug / test: fused subgrid kernel variant (dispatch_subgrid_axis.cu)
     int max_blocks;   // debug / test: cap of the persistent kernels' grid (0: none), so that a
                       // small test problem walks several lines per CTA
-    // debug / test: what the last fused subgrid launch ran (kernel, lines per CTA, output
-    // path, grid), see swiftly_b200_debug_last_launch
+    // debug / test: what the last fused subgrid, line, split or window-copy launch ran (kernel,
+    // lines per CTA or F, output path or line-fastest flag, grid), see
+    // swiftly_b200_debug_last_launch
     mutable int last_launch[4];
 };
 
@@ -41,7 +42,16 @@ const cplx* twiddles_full(const swiftly_b200* h, int n);
 // per-stream scratch of at least `samples` complex samples (grown on demand)
 cplx* split_scratch(const swiftly_b200* h, cudaStream_t s, size_t samples);
 
-// records the form of a fused subgrid launch for swiftly_b200_debug_last_launch
+// kernel codes of swiftly_b200_debug_last_launch; 1 .. 3 are the fused subgrid kernels
+// (dispatch_subgrid_axis.cu, dispatch_subgrid_split.cu)
+enum {
+    LAUNCH_LINE = 4,        // LineKernel: lines per CTA, line-fastest flag
+    LAUNCH_SPLIT_LINE = 5,  // SplitLineKernel: F = 2, flag 0
+    LAUNCH_SPLIT_F = 6,     // SplitFKernel: F, flag 0
+    LAUNCH_WINDOW_COPY = 7  // WindowCopyKernel: 0, line-fastest flag
+};
+
+// records the form of a launch for swiftly_b200_debug_last_launch (one host-side store)
 inline void note_launch(const swiftly_b200* h, int kernel, int lines, int out_path, int grid) {
     h->last_launch[0] = kernel;
     h->last_launch[1] = lines;

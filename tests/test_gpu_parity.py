@@ -176,47 +176,8 @@ def test_sdp_func_compat_adapter():
     prepare_subgrid) called the way the reference's SwiftlyCoreFunc calls it
     (core.py:577-630, 684-929), against the oracle."""
     from ska_sdp_distributed_fourier_transform_b200.sdp_func_compat import Swiftly
-    from oracle.swiftly_oracle import OracleCore, pad_mid
+    from oracle.swiftly_oracle import OracleCore
+    from tests import subgrid_line_cases as slc
 
     W, N, xM, yN, yB, xA = 13.5625, 1024, 256, 512, 416, 228
-    sw = Swiftly(N, yN, xM, W)
-    oracle = OracleCore(W, N, xM, yN)
-    m = oracle.xM_yN_size
-    rng = numpy.random.default_rng(31)
-    f_off, s_off = 12, -6
-    facet = pc.rand_c(rng, yB, 9)
-    # axis 0 through transposed views
-    out = numpy.empty((yN, 9), dtype=complex)
-    sw.prepare_facet(facet.T, out.T, f_off)
-    pc.close(out, oracle.prepare_facet(facet, f_off, axis=0), what="compat prepare_facet")
-    contrib = numpy.empty((m, 9), dtype=complex)
-    sw.extract_from_facet(out.T, contrib.T, s_off)
-    assert numpy.array_equal(contrib, oracle.extract_from_facet(out, s_off, axis=0))
-    acc = numpy.zeros((xM, 9), dtype=complex)
-    sw.add_to_subgrid(contrib.T, acc.T, f_off)
-    pc.close(acc, oracle.add_to_subgrid(contrib, f_off, axis=0), what="compat add_to_subgrid")
-    # 2-D accumulate and finish like SwiftlyCoreFunc.finish_subgrid (core.py:803-812)
-    c2 = pc.rand_c(rng, m, m)
-    acc2 = numpy.zeros((xM, xM), dtype=complex)
-    sw.add_to_subgrid_2d(c2, acc2, f_off, -f_off)
-    oacc2 = oracle.add_to_subgrid(oracle.add_to_subgrid(c2, f_off, axis=0), -f_off, axis=1)
-    pc.close(acc2, oacc2, what="compat add_to_subgrid_2d")
-    out1 = numpy.empty((xM, xA), dtype=complex)
-    sw.finish_subgrid(acc2, out1, s_off)
-    sg = numpy.empty((xA, xA), dtype=complex)
-    sw.finish_subgrid(out1.T, sg.T, -s_off)
-    pc.close(sg, oracle.finish_subgrid(oacc2, [-s_off, s_off], xA), what="compat finish_subgrid")
-    # in-place prepare_subgrid on the padded subgrid (core.py:842-853)
-    sub = pc.rand_c(rng, xA, xA)
-    padded = numpy.ascontiguousarray(pad_mid(pad_mid(sub, xM, 0), xM, 1))
-    sw.prepare_subgrid_inplace_2d(padded, s_off, -s_off)
-    pc.close(padded, oracle.prepare_subgrid(sub, (s_off, -s_off)), what="compat prepare_subgrid")
-    ext = numpy.empty((xM, m), dtype=complex)
-    sw.extract_from_subgrid(padded, ext, f_off)
-    pc.close(ext, oracle.extract_from_subgrid(padded, f_off, axis=1), what="compat extract")
-    accf = numpy.zeros((xM, yN), dtype=complex)
-    sw.add_to_facet(ext, accf, s_off)
-    assert numpy.array_equal(accf, oracle.add_to_facet(ext, s_off, axis=1))
-    fin = numpy.empty((xM, yB), dtype=complex)
-    sw.finish_facet(accf, fin, f_off)
-    pc.close(fin, oracle.finish_facet(accf, f_off, yB, axis=1), what="compat finish_facet")
+    slc.sdp_func_adapter_vs_oracle(Swiftly(N, yN, xM, W), OracleCore(W, N, xM, yN), yB, xA)
