@@ -207,11 +207,16 @@ extern "C" void swiftly_b200_debug_sg_variant(swiftly_b200* h, int variant) {
 // test hook (not in the public header): the form of the last kernel launch of the plan, so that
 // a test can assert the kernel it was written for.  out[0]: kernel (0 none yet, 1 round-1
 // SubgridAxisKernel, 2 two-group SubgridAxisKernelPP, 3 split SubgridSplitAxisKernel,
-// 4 LineKernel, 5 SplitLineKernel, 6 SplitFKernel, 7 WindowCopyKernel); out[1]: lines per CTA
-// (1 .. 4), F (5, 6: 2 for SplitLineKernel) or 0 (7); out[2]: output path of the fused kernels
-// (0 direct stores, 1 TMA with one tensor map, 2 TMA with one tensor map per group), the
-// line-fastest flag of 4 and 7, 0 for 5 and 6; out[3]: grid size.  The TMA-staged and parked
-// extract_columns forms are not recorded.
+// 4 LineKernel, 5 SplitLineKernel, 6 SplitFKernel, 7 WindowCopyKernel; the TMA-staged
+// extract_columns kernels: 8 ExtractColumnsTmaKernel<yN, false>, 9 its 2 x yN/2 split,
+// 10 ExtractColumnsTma4Kernel, 11 ExtractColumnsTmaDifKernel, 12 / 13 / 14
+// ExtractColumnsParkKernel MODE 0 / 1 / 2, 15 ExtractColumnsParkSkewKernel); out[1]: lines per
+// CTA (1 .. 4), F (5, 6: 2 for SplitLineKernel), 0 (7), or for 8 .. 15 the 128-byte chunks per
+// tensor load when the rows are staged swizzled and 0 when they are staged by linear bulk
+// copies; out[2]: output path of the fused kernels (0 direct stores, 1 TMA with one tensor map,
+// 2 TMA with one tensor map per group), the line-fastest flag of 4 and 7, 0 for 5 and 6, the
+// capacity of the staging buffer in samples for 8 .. 15; out[3]: grid size.  An extract_columns
+// launch that leaves the TMA-staged kernels records the generic kernel it ran (4, 5 or 6).
 extern "C" void swiftly_b200_debug_last_launch(const swiftly_b200* h, int* out) {
     if (h && out)
         for (int i = 0; i < 4; ++i) out[i] = h->last_launch[i];

@@ -56,9 +56,32 @@ static int launch_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op,
         k.scratch = split_scratch(h, s, (size_t)blocks * H);
         if (!k.scratch) return SWIFTLY_B200_ECUDA;
     }
+    note_launch(h, SPLIT ? LAUNCH_K2_TMA_SPLIT : LAUNCH_K2_TMA, k.swizzled ? k.box_chunks : 0,
+                k.in_cap, (int)blocks);
     cudaError_t e = launch_body_maps(k, maps, (int)blocks, smem, s);
     return e == cudaSuccess ? SWIFTLY_B200_OK : cuda_fail(e, "extract_columns (TMA) kernel launch");
 }
+
+// kernel code of swiftly_b200_debug_last_launch (plan.h)
+template <class K>
+struct K2Code;
+template <int Q>
+struct K2Code<ExtractColumnsTma4Kernel<Q>> {
+    static const int value = LAUNCH_K2_TMA4;
+};
+template <int Q, bool BOTH>
+struct K2Code<ExtractColumnsTmaDifKernel<Q, BOTH>> {
+    static const int value = LAUNCH_K2_DIF;
+};
+template <int Q, int MODE>
+struct K2Code<ExtractColumnsParkKernel<Q, MODE>> {
+    static const int value = MODE == 0 ? LAUNCH_K2_PARK_DIF
+                           : MODE == 1 ? LAUNCH_K2_PARK_DIF2 : LAUNCH_K2_PARK_DIT;
+};
+template <int Q>
+struct K2Code<ExtractColumnsParkSkewKernel<Q>> {
+    static const int value = LAUNCH_K2_PARK_SKEW;
+};
 
 // 4 x Q split with two thread groups (extract_tma.cuh)
 template <int Q, class K>
@@ -107,6 +130,7 @@ static int launch_extract_tma4(const swiftly_b200* h, const ExtractColumnsOp& op
         k.scratch = split_scratch(h, s, (size_t)blocks * scratch_lines * Q);
         if (!k.scratch) return SWIFTLY_B200_ECUDA;
     }
+    note_launch(h, K2Code<K>::value, k.swizzled ? k.box_chunks : 0, k.in_cap, (int)blocks);
     cudaError_t e = launch_body_maps(k, maps, (int)blocks, smem, s);
     return e == cudaSuccess ? SWIFTLY_B200_OK
                             : cuda_fail(e, "extract_columns (TMA, 4-way split) kernel launch");

@@ -24,9 +24,9 @@ struct swiftly_b200 {
     int sg_variant;   // debug / test: fused subgrid kernel variant (dispatch_subgrid_axis.cu)
     int max_blocks;   // debug / test: cap of the persistent kernels' grid (0: none), so that a
                       // small test problem walks several lines per CTA
-    // debug / test: what the last fused subgrid, line, split or window-copy launch ran (kernel,
-    // lines per CTA or F, output path or line-fastest flag, grid), see
-    // swiftly_b200_debug_last_launch
+    // debug / test: what the last fused subgrid, line, split, window-copy or extract_columns
+    // launch ran (kernel, lines per CTA or F or chunks per tensor load, output path or
+    // line-fastest flag or staging capacity, grid), see swiftly_b200_debug_last_launch
     mutable int last_launch[4];
 };
 
@@ -48,7 +48,18 @@ enum {
     LAUNCH_LINE = 4,        // LineKernel: lines per CTA, line-fastest flag
     LAUNCH_SPLIT_LINE = 5,  // SplitLineKernel: F = 2, flag 0
     LAUNCH_SPLIT_F = 6,     // SplitFKernel: F, flag 0
-    LAUNCH_WINDOW_COPY = 7  // WindowCopyKernel: 0, line-fastest flag
+    LAUNCH_WINDOW_COPY = 7, // WindowCopyKernel: 0, line-fastest flag
+    // the TMA-staged extract_columns kernels (dispatch_extract_columns.cu): chunks per tensor
+    // load when the rows are staged swizzled, 0 when by linear bulk copies; capacity of the
+    // staging buffer in samples
+    LAUNCH_K2_TMA = 8,         // ExtractColumnsTmaKernel<yN, false>
+    LAUNCH_K2_TMA_SPLIT = 9,   // ExtractColumnsTmaKernel<yN / 2, true>
+    LAUNCH_K2_TMA4 = 10,       // ExtractColumnsTma4Kernel<yN / 4>
+    LAUNCH_K2_DIF = 11,        // ExtractColumnsTmaDifKernel<yN / 4, BOTH>
+    LAUNCH_K2_PARK_DIF = 12,   // ExtractColumnsParkKernel<yN / 4, 0>: facets of at most yN / 2
+    LAUNCH_K2_PARK_DIF2 = 13,  // ExtractColumnsParkKernel<yN / 4, 1>: longer facets
+    LAUNCH_K2_PARK_DIT = 14,   // ExtractColumnsParkKernel<yN / 4, 2>
+    LAUNCH_K2_PARK_SKEW = 15   // ExtractColumnsParkSkewKernel<yN / 4>
 };
 
 // records the form of a launch for swiftly_b200_debug_last_launch (one host-side store)

@@ -127,6 +127,12 @@ bool make_row_map(TensorMap4* tm, const cplx* base, int64_t ls, int64_t n_rows, 
 }
 
 #if defined(SWIFTLY_EMU)
+// the bytes a tensor load reports to its mbarrier: the whole box, the zero fill outside the tensor
+// included
+uint32_t emu_tensor_box_bytes(const TensorMap4* tm) {
+    return (uint32_t)(tm->box[0] * tm->box[1] * tm->box[2] * tm->box[3]) * (uint32_t)sizeof(double);
+}
+
 // what the TMA engine does with a (128-byte swizzled) tensor load of box (0, c1, c2, 0)
 void emu_tensor_load(const TensorMap4* tm, double* dst, int c1, int c2) {
     for (int i1 = 0; i1 < tm->box[1]; ++i1)

@@ -89,15 +89,13 @@ struct HostCtx {
     inline void group_sync(int id, int count) const;
     inline void group_arrive(int id, int count) const;
     inline void yield() const;
-    // bulk asynchronous copies: the emulated copy completes immediately (races between the
-    // asynchronous copy and ordinary accesses are NOT modelled -- only the index algebra is)
-    inline void tx_init(uint64_t* bar) const { *bar = 0; }
-    inline void tx_expect(uint64_t*, uint32_t) const {}
-    inline void tx_copy(void* dst, const void* src, uint32_t bytes, uint64_t* bar) const {
-        memcpy(dst, src, bytes);
-        *bar += 1;
-    }
-    inline void tx_wait(uint64_t*, uint32_t) const {}
+    // bulk asynchronous copies tracked by an mbarrier: the emulated copy completes immediately
+    // (races between the asynchronous copy and ordinary accesses are NOT modelled), but the
+    // barrier's transaction protocol is accounted for, see EmuTxBarrier below
+    inline void tx_init(uint64_t* bar) const;
+    inline void tx_expect(uint64_t* bar, uint32_t bytes) const;
+    inline void tx_copy(void* dst, const void* src, uint32_t bytes, uint64_t* bar) const;
+    inline void tx_wait(uint64_t* bar, uint32_t parity) const;
     inline void bulk_prefetch_l2(const void*, uint32_t) const {}
     inline void nap(unsigned) const {}
     inline void fence_async() const {}
@@ -116,17 +114,36 @@ namespace swiftly {
 struct TensorMap4;
 void emu_tensor_store(const TensorMap4* map, const double* src, int c1, int c2, int c3);
 void emu_tensor_load(const TensorMap4* map, double* dst, int c1, int c2);
-inline void HostCtx::tensor_load(void* smem_dst, const void* map, int c1, int c2,
-                                 uint64_t* bar) const {
-    emu_tensor_load((const TensorMap4*)map, (double*)smem_dst, c1, c2);
-    *bar += 1;
-}
+// the bytes a load delivers: the full box, zero fill included
+uint32_t emu_tensor_box_bytes(const TensorMap4* map);
 inline void HostCtx::tensor_store(const void* map, const void* smem_src, int c1, int c2,
                                   int c3) const {
     emu_tensor_store((const TensorMap4*)map, (const double*)smem_src, c1, c2, c3);
 }
 
+// State of one bulk-copy barrier (an mbarrier initialised with count 1, as DeviceCtx::tx_init
+// does) of the running CTA.  The hardware completes a phase when the arming thread has arrived
+// (tx_expect) and the bytes it announced have been delivered; a wait on parity p returns once the
+// phase of that parity is complete.  A protocol slip therefore hangs the CTA or lets it read a
+// row that has not landed.  The emulator reports instead:
+//   * tx_expect on a barrier whose current phase is already armed;
+//   * a copy arriving on a barrier that is not armed, or delivering more bytes than are left;
+//   * tx_wait with the wrong parity -- every thread of the CTA waits on every phase once, in
+//     order (so do all kernels of the library), hence a thread's k-th wait takes parity k & 1;
+//   * tx_wait on a phase that is not complete: the emulated copies are synchronous, so bytes
+//     still missing when the wait is reached never arrive;
+//   * a phase completing while some thread has not yet waited on the phase before it: that
+//     thread's wait would be answered by the wrong phase.
+struct EmuTxBarrier {
+    uint64_t* bar;
+    bool armed;
+    uint32_t pending;             // bytes the current phase still expects
+    unsigned phases;              // completed phases
+    std::vector<unsigned> waits;  // per thread: waits done
+};
+
 struct EmuBlock {
+    std::vector<EmuTxBarrier> tx;
     ucontext_t main_ctx;
     std::vector<ucontext_t> ctxs;
     std::vector<char*> stacks;
@@ -161,6 +178,74 @@ static inline void emu_check_barrier(int id, int count, int cta_threads) {
                         "take ids 0..15 and whole warps\n", id, count);
         abort();
     }
+}
+
+static inline void emu_tx_error(const HostCtx& c, const char* what, const EmuTxBarrier* b) {
+    fprintf(stderr, "swiftly emulator: bulk-copy barrier PROTOCOL error in block %d, thread %d: %s",
+            c.bid, c.tid, what);
+    if (b)
+        fprintf(stderr, " (%u phases complete, current phase %s, %u bytes outstanding)", b->phases,
+                b->armed ? "armed" : "not armed", b->pending);
+    fprintf(stderr, "\n");
+    abort();
+}
+
+static inline EmuTxBarrier& emu_tx_find(const HostCtx& c, uint64_t* bar) {
+    for (EmuTxBarrier& b : c.blk->tx)
+        if (b.bar == bar) return b;
+    emu_tx_error(c, "barrier used before tx_init", nullptr);
+    abort();
+}
+
+static inline void emu_tx_deliver(const HostCtx& c, uint64_t* bar, uint32_t bytes) {
+    EmuTxBarrier& b = emu_tx_find(c, bar);
+    if (!b.armed) emu_tx_error(c, "copy arrives on a barrier that is not armed", &b);
+    if (bytes > b.pending) emu_tx_error(c, "copy delivers more bytes than tx_expect announced", &b);
+    b.pending -= bytes;
+    if (b.pending) return;
+    for (unsigned w : b.waits)
+        if (w < b.phases)
+            emu_tx_error(c, "phase completes before every thread waited on the previous one", &b);
+    b.armed = false;
+    ++b.phases;
+}
+
+inline void HostCtx::tx_init(uint64_t* bar) const {
+    EmuTxBarrier fresh{bar, false, 0, 0, std::vector<unsigned>(blk->nthreads, 0u)};
+    for (EmuTxBarrier& b : blk->tx)
+        if (b.bar == bar) {
+            b = fresh;
+            return;
+        }
+    blk->tx.push_back(fresh);
+}
+
+inline void HostCtx::tx_expect(uint64_t* bar, uint32_t bytes) const {
+    EmuTxBarrier& b = emu_tx_find(*this, bar);
+    if (b.armed) emu_tx_error(*this, "tx_expect on a phase that is already armed", &b);
+    b.armed = true;
+    b.pending = bytes;
+    if (!bytes) emu_tx_deliver(*this, bar, 0);
+}
+
+inline void HostCtx::tx_copy(void* dst, const void* src, uint32_t bytes, uint64_t* bar) const {
+    memcpy(dst, src, bytes);
+    emu_tx_deliver(*this, bar, bytes);
+}
+
+inline void HostCtx::tensor_load(void* smem_dst, const void* map, int c1, int c2,
+                                 uint64_t* bar) const {
+    emu_tensor_load((const TensorMap4*)map, (double*)smem_dst, c1, c2);
+    emu_tx_deliver(*this, bar, emu_tensor_box_bytes((const TensorMap4*)map));
+}
+
+inline void HostCtx::tx_wait(uint64_t* bar, uint32_t parity) const {
+    EmuTxBarrier& b = emu_tx_find(*this, bar);
+    const unsigned k = b.waits[tid];
+    if ((k & 1u) != (parity & 1u))
+        emu_tx_error(*this, "tx_wait with the parity of the wrong phase", &b);
+    if (b.phases <= k) emu_tx_error(*this, "tx_wait on a phase that cannot complete", &b);
+    b.waits[tid] = k + 1;
 }
 
 inline void HostCtx::group_arrive(int id, int count) const {
@@ -241,6 +326,7 @@ inline cudaError_t launch_body_impl(const Body& body, const void* tmaps, int gri
         }
         g_emu_block = &blk;
         blk.nthreads = T;
+        blk.tx.clear();
         for (int i = 0; i < 16; ++i) {
             blk.bar_arrived[i] = 0;
             blk.bar_gen[i] = 0;

@@ -227,40 +227,14 @@ def test_k2_kernel_forms_yN16384(sg_variant):
     per thread in L2-resident scratch, DIT within and across the two thread groups, store phases
     half a line apart, 18 = without the skew, 17 = DIF across the groups with 32-byte pair
     stores, 15 = DIF / DIT with the L2 scratch, 7 = 2 x 8192.  Rows staged by swizzled tensor loads (fs = 8192),
-    by linear bulk copies (odd fs), rows longer than yN / 2, several lines per CTA."""
-    import ctypes
-
+    by linear bulk copies (odd fs), rows longer than yN / 2, several lines per CTA; each launch
+    asserts the kernel it recorded (tests/k2_cases.py::variant_case)."""
     from oracle.swiftly_oracle import OracleCore
+    from tests import k2_cases
 
     W, N, yN, xM = 13.5625, 65536, 16384, 4096
     cfg = make_config(W, N, 8192, yN, 2048, xM)
-    core = cfg.core
-    core._lib.swiftly_b200_debug_sg_variant.argtypes = [ctypes.c_void_p, ctypes.c_int]
-    core._lib.swiftly_b200_debug_sg_variant(core._plan, sg_variant)
-    oracle = OracleCore(W, N, xM, yN)
-    m = core.xM_yN_size
-    rng = numpy.random.default_rng(16384 + sg_variant)
-    dev = torch.device("cuda")
-    sg_off0 = 3 * 2048
-    # (only the m rows the subgrid column takes are filled on the host: the oracle needs just them)
-    rows = numpy.unique(oracle._facet_window(sg_off0))
-    assert rows.size == m
-    for sizes, offs in (((8192, 8192), (8192, -16384)), ((8191, 9000), (0, 24576))):
-        bfs, refs = [], []
-        for fs, off1 in zip(sizes, offs):
-            bf = torch.zeros(yN, fs, dtype=torch.complex128, device=dev)
-            blk = pc.rand_c(rng, m, fs)
-            bf[torch.from_numpy(rows).to(dev)] = torch.from_numpy(blk).to(dev)
-            bfs.append(bf)
-            full = numpy.zeros((yN, fs), dtype=complex)
-            full[rows] = blk
-            refs.append(oracle.prepare_facet(oracle.extract_from_facet(full, sg_off0, axis=0),
-                                             off1, axis=1))
-        outs = core.extract_columns(bfs, sg_off0, list(offs))
-        for o, r in zip(outs, refs):
-            assert numpy.abs(o.cpu().numpy() - r).max() <= 1e-12 * numpy.abs(r).max()
-        del bfs, outs
-    core._lib.swiftly_b200_debug_sg_variant(core._plan, 0)
+    k2_cases.variant_case(cfg.core, OracleCore(W, N, xM, yN), sg_variant, seed=16384 + sg_variant)
 
 
 def test_cfg4_full_size_properties():
