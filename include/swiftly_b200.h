@@ -182,8 +182,17 @@ int swiftly_b200_peer_signal(const swiftly_b200* plan, void* const* flags_dev_ta
                              int my_rank, int64_t value, void* stream);
 int swiftly_b200_peer_wait(const swiftly_b200* plan, const void* my_flags, int n_peers,
                            int64_t value, double timeout_s, void* status, void* stream);
+/* Row rings.  A subgrid column reads (extract_columns) or adds into (fold_column) only an
+ * xM_yN_size-row window of each yN_size-row facet array: rows (yN/2 - m/2 + s) mod yN + u,
+ * u < m, with m = xM_yN_size and s = subgrid_off0 * yN_size // N.  Instead of the whole array
+ * a caller may pass a RING of m rows: facet row r lives at ring line r mod m (m divides yN, so
+ * the mapping holds across the wrap at yN).  The ring must hold the window's rows of the
+ * column at hand; rows that stay when the window slides keep their line.  In one call every
+ * bf_f[f] (every facet_accs[f]) has yN_size lines, or every one has xM_yN_size lines; any other
+ * line count is rejected.  A ring runs the same kernel form as the whole array with the same
+ * facet size and row stride. */
 /* swiftly_b200_extract_column for n_facets (<= 64) facets in ONE launch: bf_f[f] / out[f]
- * as in swiftly_b200_extract_column (contiguous rows), facet_off1[f] per facet. */
+ * as in swiftly_b200_extract_column (contiguous rows, or row rings), facet_off1[f] per facet. */
 int swiftly_b200_extract_columns(const swiftly_b200* plan, int n_facets,
                                  const swiftly_b200_lines* bf_f, const swiftly_b200_lines* out,
                                  int64_t subgrid_off0, const int64_t* facet_off1, void* stream);
@@ -212,7 +221,8 @@ int swiftly_b200_subgrid_to_facets(const swiftly_b200* plan, int n_facets,
 /* Fold a finished subgrid column into n_facets facet accumulators in ONE launch: per facet
  * `finish_facet(acc, facet_off1, size, axis=1)`, optional mask1, `add_to_facet(., subgrid_off0,
  * axis=0, out=facet_acc)` (api_helper.py:155-179).  facet_accs[f]: (yN_size x facet_size)
- * accumulator MNAF_BMNAF, ACCUMULATED into; mask1 or mask1[f] may be NULL. */
+ * accumulator MNAF_BMNAF (or its row ring, see "Row rings" above), ACCUMULATED into; mask1 or
+ * mask1[f] may be NULL. */
 int swiftly_b200_fold_column(const swiftly_b200* plan, int n_facets,
                              const swiftly_b200_lines* accs,
                              const swiftly_b200_lines* facet_accs, const int64_t* facet_off1,

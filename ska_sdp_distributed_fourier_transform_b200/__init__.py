@@ -9,10 +9,12 @@ behind a C ABI (``include/swiftly_b200.h``).  No CPU fallback.
 
 from .api import (  # noqa: F401
     FacetConfig,
+    PinnedArena,
     SubgridConfig,
     SwiftlyBackward,
     SwiftlyConfig,
     SwiftlyForward,
+    device_tier_bytes,
     make_full_facet_cover,
     make_full_subgrid_cover,
 )
@@ -29,6 +31,7 @@ from .swift_configs import SWIFT_CONFIGS  # noqa: F401
 
 __all__ = [
     "FacetConfig",
+    "PinnedArena",
     "SubgridConfig",
     "SwiftlyConfig",
     "SwiftlyForward",
@@ -38,6 +41,7 @@ __all__ = [
     "SwiftlyBackwardSharded",
     "partition_facets",
     "SWIFT_CONFIGS",
+    "device_tier_bytes",
     "check_facet",
     "check_subgrid",
     "make_subgrid",

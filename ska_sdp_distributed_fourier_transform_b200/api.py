@@ -17,6 +17,7 @@ in flight.  ``dask_client`` / ``client`` are accepted and ignored.
 
 import collections
 import logging
+import time
 
 import numpy
 
@@ -43,6 +44,8 @@ __all__ = [
     "SwiftlyConfig",
     "SwiftlyForward",
     "SwiftlyBackward",
+    "PinnedArena",
+    "device_tier_bytes",
     "make_full_facet_cover",
     "make_full_subgrid_cover",
 ]
@@ -336,6 +339,187 @@ def _upload_iter(datas, device):
         yield t
 
 
+# ---------------------------------------------------------------------- host tier
+def device_tier_bytes(direction, yN, m, facet_sizes, lru, n_rows=0, subgrid_size=0):
+    """Bytes of device memory the device tier of a one-GPU transform holds at its peak.
+
+    ``"forward"``: every prepared facet ``BF_F`` (``yN x size``), ``lru`` subgrid columns of
+    ``NMBF_BF`` (``m x yN`` per facet), the subgrid strips (``n_rows x m x subgrid_size``) and the
+    stage-1 scratch (one ``yN x size`` facet).  ``"backward"``: every facet accumulator
+    (``yN x size``) and ``lru`` columns of accumulators (``m x yN`` per facet).  When this exceeds
+    the device budget, :class:`SwiftlyForward` / :class:`SwiftlyBackward` keep those facet arrays
+    in pinned host memory instead (the host tier).
+    """
+    sizes = list(facet_sizes)
+    facets = 16 * yN * sum(sizes)
+    columns = 16 * max(1, int(lru)) * len(sizes) * m * yN
+    if direction == "backward":
+        return facets + columns
+    if direction != "forward":
+        raise ValueError(f"direction must be 'forward' or 'backward', not {direction!r}")
+    return facets + columns + 16 * n_rows * m * subgrid_size + 16 * yN * max(sizes, default=0)
+
+
+def _device_budget(device, device_budget):
+    """``device_budget`` if given, else the free memory of ``device`` (no limit on the CPU
+    "device" of the emulated library)."""
+    if device_budget is not None:
+        return int(device_budget)
+    if device.type != "cuda":
+        return float("inf")
+    return torch.cuda.mem_get_info(device)[0]
+
+
+def window_start(core, subgrid_off0):
+    """First row of the ``m``-row window of the ``yN``-row facet arrays that subgrid column
+    ``subgrid_off0`` reads (forward) or adds into (backward); the window wraps modulo ``yN``."""
+    yN, m = core.yN_size, core.xM_yN_size
+    return (yN // 2 - m // 2 + (subgrid_off0 * yN) // core.N) % yN
+
+
+class _RowWindow:
+    """The ``m``-row window of the ``yN``-row facet arrays that the device rings hold.  Facet row
+    ``r`` lives at ring line ``r mod m`` (``m`` divides ``yN``), so rows that stay when the window
+    slides keep their line and each new row takes the line of a row that left."""
+
+    def __init__(self, yN, m):
+        self.yN = yN
+        self.m = m
+        self.start = None
+
+    def rows(self, start):
+        return [(start + u) % self.yN for u in range(self.m)]
+
+    def move(self, start):
+        """Slide to the window at ``start``; returns ``(leaving, entering)`` rows."""
+        old = [] if self.start is None else self.rows(self.start)
+        new = self.rows(start)
+        self.start = start
+        old_set, new_set = set(old), set(new)
+        return [r for r in old if r not in new_set], [r for r in new if r not in old_set]
+
+    def runs(self, rows):
+        """``(first row, count)`` of the runs of consecutive ``rows`` that are also consecutive ring
+        lines: a run ends at every multiple of ``m``, so also at the wrap at ``yN``."""
+        out = []
+        for r in rows:
+            if out and r == out[-1][0] + out[-1][1] and r % self.m:
+                out[-1][1] += 1
+            else:
+                out.append([r, 1])
+        return [(r, n) for r, n in out]
+
+
+class _Copier:
+    """Copies between host memory and the device on one copy stream, ordered against the compute
+    stream by events.  On the emulated library's CPU "device" every copy runs at once."""
+
+    def __init__(self, device):
+        self.device = device
+        self.stream = torch.cuda.Stream(device) if device.type == "cuda" else None
+        self.h2d_bytes = 0
+        self.d2h_bytes = 0
+
+    def _compute(self):
+        return torch.cuda.current_stream(self.device)
+
+    def use(self, t):
+        """``t`` (a device tensor) is used on the copy stream: keep its memory until then."""
+        if self.stream is not None:
+            t.record_stream(self.stream)
+        return t
+
+    def record(self, on_copy=True):
+        """Event after the work queued so far on the copy (or compute) stream; None on the CPU."""
+        if self.stream is None:
+            return None
+        ev = torch.cuda.Event()
+        ev.record(self.stream if on_copy else self._compute())
+        return ev
+
+    def copy_waits(self, ev):
+        if ev is not None:
+            self.stream.wait_event(ev)
+
+    def compute_waits(self, ev):
+        if ev is not None:
+            self._compute().wait_event(ev)
+
+    def after_compute(self):
+        """Later copies wait for everything queued so far on the compute stream."""
+        self.copy_waits(self.record(on_copy=False))
+
+    def copy(self, dst, src, to_host):
+        """Queue ``dst.copy_(src)``: device -> host if ``to_host``, else host -> device."""
+        nbytes = src.numel() * src.element_size()
+        if to_host:
+            self.d2h_bytes += nbytes
+        else:
+            self.h2d_bytes += nbytes
+        if self.stream is None:
+            dst.copy_(src)
+            return
+        with torch.cuda.stream(self.stream):
+            dst.copy_(src, non_blocking=True)
+
+    def zero(self, t):
+        if self.stream is None:
+            t.zero_()
+            return
+        with torch.cuda.stream(self.stream):
+            t.zero_()
+
+    def synchronize(self):
+        if self.stream is not None:
+            self.stream.synchronize()
+
+
+class PinnedArena:
+    """One page-locked host allocation, cut into ``(rows, size)`` complex128 views.
+
+    The memory is a plain CPU tensor registered with ``cudaHostRegister`` (torch's caching host
+    allocator would round the block size up).  On the emulated library's CPU "device" it stays
+    pageable.  ``seconds`` is the time allocation and pinning took.  Views handed out stay valid
+    after :meth:`release` (the memory is then pageable until the last view goes).
+    """
+
+    def __init__(self, shapes, device):
+        t0 = time.perf_counter()
+        self.shapes = [tuple(int(d) for d in s) for s in shapes]
+        total = sum(a * b for a, b in self.shapes)
+        self.tensor = torch.empty(max(1, total), dtype=torch.complex128)
+        self.nbytes = self.tensor.numel() * 16
+        self._registered = False
+        if device.type == "cuda":
+            with torch.cuda.device(device):
+                torch.cuda.check_error(torch.cuda.cudart().cudaHostRegister(
+                    self.tensor.data_ptr(), self.nbytes, 0))
+            self._registered = True
+        self.seconds = time.perf_counter() - t0
+        self.views = []
+        off = 0
+        for a, b in self.shapes:
+            self.views.append(self.tensor[off:off + a * b].view(a, b))
+            off += a * b
+
+    def release(self):
+        """Unpin the memory (idempotent)."""
+        if self._registered:
+            self._registered = False
+            torch.cuda.cudart().cudaHostUnregister(self.tensor.data_ptr())
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:  # pylint: disable=broad-except
+            pass
+
+
+# facets per K2 launch of the forward host tier: the H2D copy of the next batch's new ring rows
+# overlaps K2 of this batch
+RING_BATCH = 8
+
+
 def _device_mask(mask, device):
     """float64 device mask, or None when the mask is absent or all ones."""
     if mask is None:
@@ -357,14 +541,20 @@ class SwiftlyForward:
         (``NMBF_BF``) stay resident
     :param queue_size: maximum number of unfinished subgrid results
     :param client: accepted for compatibility, ignored
-    :param bf_f_buffers: optional preallocated ``(yN, size)`` device tensors that
-        receive the axis-0 prepared facets (they may reuse storage of facets that
-        were consumed earlier in the list; facets are processed in list order)
+    :param bf_f_buffers: optional preallocated ``(yN, size)`` tensors that receive the
+        axis-0 prepared facets.  Device tensors may reuse storage of facets that were
+        consumed earlier in the list (facets are processed in list order); host tensors
+        (ideally pinned, e.g. the views of a :class:`PinnedArena`) select the host tier
+    :param device_budget: bytes of device memory the transform may use (default: the
+        device's free memory now).  When the device tier needs more
+        (:func:`device_tier_bytes`), the prepared facets live in pinned host memory and
+        each subgrid column brings only its ``m``-row window of them to the device (the
+        host tier); the subgrids are the same bits either way
     """
 
     # pylint: disable=too-many-arguments,too-many-instance-attributes
     def __init__(self, swiftly_config, facet_tasks, lru_forward=1, queue_size=20, client=None,
-                 bf_f_buffers=None):
+                 bf_f_buffers=None, device_budget=None):
         self.config = swiftly_config
         self.facet_tasks = list(facet_tasks)
         self.core = swiftly_config.core
@@ -385,9 +575,64 @@ class SwiftlyForward:
         self._prep1 = None
         self._masks = {}
         self._fused = bool(getattr(self.core, "fused_forward_supported", lambda: False)())
+        self.host_tier = self._fused and self._select_host_tier(device_budget)
+        self.arena = None
+        self._rings = None
+        self._ring_k2 = None
+        self._window = None
+        # rows of the m-row window copied host -> device in stage 2 (per facet)
+        self.h2d_rows = 0
+        self._copier = _Copier(self.device) if self.host_tier else None
+
+    def _select_host_tier(self, device_budget):
+        if self._bf_f_buffers is not None:
+            return self._bf_f_buffers[0].device != self.device
+        if not self.facet_tasks:
+            return False
+        core = self.core
+        sizes = [cfg.size for cfg, _ in self.facet_tasks]
+        need = device_tier_bytes("forward", core.yN_size, core.xM_yN_size, sizes, self.lru.size,
+                                 len(self._rows), self.config.max_subgrid_size)
+        return need > _device_budget(self.device, device_budget)
+
+    @property
+    def copied_bytes(self):
+        """``(host -> device, device -> host)`` bytes the host tier moved so far."""
+        cp = self._copier
+        return (cp.h2d_bytes, cp.d2h_bytes) if cp is not None else (0, 0)
 
     # -- stage 1: prepare every facet along axis 0 (once) --------------------------------
+    def _stage1_host(self):
+        """K1 into two device buffers in turn; the copy stream moves each finished buffer to the
+        facet's host ``BF_F`` while K1 prepares the next facet.  K1 of facet ``j + 2`` waits for
+        the copy of facet ``j``."""
+        core, cp = self.core, self._copier
+        yN = core.yN_size
+        sizes = [cfg.size for cfg, _ in self.facet_tasks]
+        if self._bf_f_buffers is not None:
+            hosts = list(self._bf_f_buffers)
+        else:
+            self.arena = PinnedArena([(yN, s) for s in sizes], self.device)
+            hosts = self.arena.views
+        stage = cp.use(torch.empty((2, yN * max(sizes)), dtype=torch.complex128,
+                                   device=self.device))
+        copied = [None, None]
+        uploads = _upload_iter([data for _, data in self.facet_tasks], self.device)
+        for idx, ((cfg, _), facet) in enumerate(zip(self.facet_tasks, uploads)):
+            slot = idx % 2
+            cp.compute_waits(copied[slot])
+            buf = stage[slot, :yN * cfg.size].view(yN, cfg.size)
+            core.prepare_facet(facet, cfg.off0, axis=0, out=buf, window_lines=True)
+            del facet
+            cp.after_compute()
+            cp.copy(hosts[idx], buf, True)
+            copied[slot] = cp.record()
+        return hosts
+
     def _get_BF_Fs(self):
+        if self.BF_Fs_persist is None and self.host_tier:
+            self.BF_Fs_persist = self._stage1_host()
+            self.facet_tasks = [(cfg, None) for cfg, _ in self.facet_tasks]
         if self.BF_Fs_persist is None:
             out = []
             uploads = _upload_iter([data for _, data in self.facet_tasks], self.device)
@@ -417,7 +662,9 @@ class SwiftlyForward:
             if len(self.lru.data) >= self.lru.size:
                 # recycle the buffers of the column that is about to be evicted
                 _, reuse = self.lru.data.popitem(last=False)
-            if self._fused:
+            if self.host_tier:
+                cached = self._columns_from_rings(BF_Fs, off0, reuse)
+            elif self._fused:
                 cached = self.core.extract_columns(
                     BF_Fs, off0, [cfg.off1 for cfg, _ in self.facet_tasks], outs=reuse,
                     prewindowed=True)
@@ -426,6 +673,38 @@ class SwiftlyForward:
                           for (cfg, _), BF_F in zip(self.facet_tasks, BF_Fs)]
             self.lru.set(off0, cached)
         return cached
+
+    def _columns_from_rings(self, hosts, off0, outs):
+        """K2 of the host tier: every facet has a device ring of ``m`` rows; the rows of the
+        column's window that the rings lack are copied from the host ``BF_F`` (the copy of batch
+        ``b + 1`` overlaps K2 of batch ``b``), then K2 reads the rings."""
+        core, cp = self.core, self._copier
+        m, yN = core.xM_yN_size, core.yN_size
+        n = len(hosts)
+        if self._rings is None:
+            self._rings = [cp.use(torch.empty((m, h.shape[1]), dtype=torch.complex128,
+                                              device=self.device)) for h in hosts]
+            self._ring_k2 = [None] * len(range(0, n, RING_BATCH))
+            self._window = _RowWindow(yN, m)
+        _, entering = self._window.move(window_start(core, off0))
+        runs = self._window.runs(entering)
+        self.h2d_rows += len(entering)
+        if outs is None:
+            outs = [torch.empty((m, yN), dtype=torch.complex128, device=self.device)
+                    for _ in hosts]
+        off1s = [cfg.off1 for cfg, _ in self.facet_tasks]
+        for b, lo in enumerate(range(0, n, RING_BATCH)):
+            hi = min(lo + RING_BATCH, n)
+            # the ring lines about to be overwritten were last read by K2 of this batch
+            cp.copy_waits(self._ring_k2[b])
+            for j in range(lo, hi):
+                for r0, cnt in runs:
+                    cp.copy(self._rings[j][r0 % m:r0 % m + cnt], hosts[j][r0:r0 + cnt], False)
+            cp.compute_waits(cp.record())
+            core.extract_columns(self._rings[lo:hi], off0, off1s[lo:hi], outs=outs[lo:hi],
+                                 prewindowed=True)
+            self._ring_k2[b] = cp.record(on_copy=False)
+        return outs
 
     # -- stage 3: per subgrid ---------------------------------------------------------------
     def _gen_subgrid(self, subgrid_config, NMBF_BFs):
@@ -494,11 +773,16 @@ class SwiftlyBackward:
         (``NAF_MNAF``) stay resident before they are folded into the facets
     :param queue_size: maximum number of unfinished results
     :param client: accepted for compatibility, ignored
+    :param device_budget: bytes of device memory the transform may use (default: the
+        device's free memory now).  When the device tier needs more
+        (:func:`device_tier_bytes`), the facet accumulators live in pinned host memory and
+        the device holds only the ``m``-row window the current column adds into (the host
+        tier); ``finish()`` then returns the facets in pinned host memory, the same bits
     """
 
-    # pylint: disable=too-many-arguments
+    # pylint: disable=too-many-arguments,too-many-instance-attributes
     def __init__(self, swiftly_config, facets_config_list, lru_backward=1, queue_size=20,
-                 client=None):
+                 client=None, device_budget=None):
         self.config = swiftly_config
         self.core = swiftly_config.core
         self.device = _device_of(self.core)
@@ -524,6 +808,106 @@ class SwiftlyBackward:
         self._row_members = dict(self._rows)
         self._strips = None
         self._masks1 = None
+        self.host_tier = self._fused and bool(self.facets_config_list) and device_tier_bytes(
+            "backward", self.core.yN_size, self.core.xM_yN_size,
+            [cfg.size for cfg in self.facets_config_list], self.lru.size,
+        ) > _device_budget(self.device, device_budget)
+        self.arena = None
+        self._rings = None
+        self._window = None
+        self._touched = None  # per facet row: written back to the host accumulators yet
+        # rows of the m-row window moved per facet: host -> device, device -> host, zero-filled
+        self.h2d_rows = 0
+        self.d2h_rows = 0
+        self.zeroed_rows = 0
+        self._copier = _Copier(self.device) if self.host_tier else None
+
+    @property
+    def copied_bytes(self):
+        """``(host -> device, device -> host)`` bytes the host tier moved so far."""
+        cp = self._copier
+        return (cp.h2d_bytes, cp.d2h_bytes) if cp is not None else (0, 0)
+
+    def _write_back(self, rows):
+        """Queue the D2H copy of ``rows`` (held by the rings) to the host accumulators."""
+        cp, m = self._copier, self.core.xM_yN_size
+        for r0, cnt in self._window.runs(rows):
+            for ring, host in zip(self._rings, self.arena.views):
+                cp.copy(host[r0:r0 + cnt], ring[r0 % m:r0 % m + cnt], True)
+        self._touched[rows] = True
+        self.d2h_rows += len(rows)
+
+    def _load_rows(self, rows, targets, line_of):
+        """Queue the rows of the host accumulators into ``targets`` (line ``line_of(r)`` for row
+        ``r``): copied if a column wrote them back before, zero-filled otherwise."""
+        cp = self._copier
+        touched = [r for r in rows if self._touched[r]]
+        fresh = [r for r in rows if not self._touched[r]]
+        for r0, cnt in self._window.runs(touched):
+            for t, host in zip(targets, self.arena.views):
+                cp.copy(t[line_of(r0):line_of(r0) + cnt], host[r0:r0 + cnt], False)
+        for r0, cnt in self._window.runs(fresh):
+            for t in targets:
+                cp.zero(t[line_of(r0):line_of(r0) + cnt])
+        self.h2d_rows += len(touched)
+        self.zeroed_rows += len(fresh)
+
+    def _slide_rings(self, off0):
+        """Make the rings hold the window of subgrid column ``off0``: rows that leave go back to
+        the host after the folds queued so far, then rows that enter are loaded, all on one copy
+        stream (a row written back is never read back before it lands)."""
+        core, cp = self.core, self._copier
+        m, yN = core.xM_yN_size, core.yN_size
+        if self._rings is None:
+            self.arena = PinnedArena([(yN, cfg.size) for cfg in self.facets_config_list],
+                                     self.device)
+            self._rings = [cp.use(torch.empty((m, cfg.size), dtype=torch.complex128,
+                                              device=self.device))
+                           for cfg in self.facets_config_list]
+            self._window = _RowWindow(yN, m)
+            self._touched = numpy.zeros(yN, dtype=bool)
+        start = window_start(core, off0)
+        if start == self._window.start:
+            return
+        leaving, entering = self._window.move(start)
+        cp.after_compute()
+        if leaving:
+            self._write_back(leaving)
+        self._load_rows(entering, self._rings, lambda r: r % m)
+        cp.compute_waits(cp.record())
+
+    def _finish_host(self):
+        """Flush the rings, then per facet: the accumulator into one reused ``yN x size`` device
+        buffer, ``finish_facet`` along axis 0, the facet back into pinned host memory (the start
+        of the facet's own, no longer needed, accumulator)."""
+        core, cp = self.core, self._copier
+        yN = core.yN_size
+        tasks = []
+        if self._rings is None:  # no column was folded: every accumulator is zero
+            self._slide_rings(0)
+        cp.after_compute()
+        self._write_back(self._window.rows(self._window.start))
+        self._rings = None
+        sizes = [cfg.size for cfg in self.facets_config_list]
+        buf = cp.use(torch.empty(yN * max(sizes), dtype=torch.complex128, device=self.device))
+        touched = self._window.runs([r for r in range(yN) if self._touched[r]])
+        fresh = self._window.runs([r for r in range(yN) if not self._touched[r]])
+        for j, cfg in enumerate(self.facets_config_list):
+            acc = buf[:yN * cfg.size].view(yN, cfg.size)
+            host = self.arena.views[j]
+            cp.after_compute()  # the previous facet's finish_facet has read the buffer
+            for r0, cnt in touched:
+                cp.copy(acc[r0:r0 + cnt], host[r0:r0 + cnt], False)
+            for r0, cnt in fresh:
+                cp.zero(acc[r0:r0 + cnt])
+            cp.compute_waits(cp.record())
+            facet = finish_facet(core, acc, cfg)
+            out = host.reshape(-1)[:cfg.size * cfg.size].view(cfg.size, cfg.size)
+            cp.after_compute()
+            cp.copy(out, cp.use(facet), True)
+            tasks.append(DeviceTask(out))
+        cp.synchronize()
+        return tasks
 
     def add_new_subgrid_task(self, subgrid_config, new_subgrid_task):
         """Fold one subgrid into the facet accumulators."""
@@ -629,6 +1013,15 @@ class SwiftlyBackward:
 
     def update_MNAF_BMNAFs(self, off0, new_NAF_MNAFs):
         """Finish a subgrid column along axis 1 and fold it into the facets (axis 0)."""
+        if self.host_tier:
+            if self._masks1 is None:
+                self._masks1 = [_device_mask(cfg.mask1, self.device)
+                                for cfg in self.facets_config_list]
+            self._slide_rings(off0)
+            self.core.fold_column(new_NAF_MNAFs, self._rings,
+                                  [cfg.off1 for cfg in self.facets_config_list], self._masks1,
+                                  off0)
+            return self._rings
         if self._fused:
             core = self.core
             for j, cfg in enumerate(self.facets_config_list):
@@ -653,6 +1046,8 @@ class SwiftlyBackward:
         """Flush all pending columns and finish the facets; returns result handles."""
         for old_off0, old_column in self.lru.pop_all():
             self.update_MNAF_BMNAFs(old_off0, old_column)
+        if self.host_tier:
+            return self._finish_host()
         tasks = []
         for j, cfg in enumerate(self.facets_config_list):
             # release every accumulator as soon as its facet is finished: (yN, size) goes,

@@ -463,6 +463,9 @@ class SwiftlyCoreB200:
         """``extract_column`` for a list of facets in ONE kernel launch (<= 64 per launch).
 
         ``prewindowed``: the ``BF_Fs`` were made with ``prepare_facet(..., window_lines=True)``.
+        Every ``BF_F`` is a whole ``(yN_size, size)`` prepared facet, or every one is an
+        ``(xM_yN_size, size)`` row ring holding row ``r`` of the column's window at line
+        ``r mod xM_yN_size`` (include/swiftly_b200.h, "Row rings").
         """
         shape = (self.xM_yN_size, self.yN_size)
         BF_Fs = list(BF_Fs)
@@ -769,8 +772,10 @@ class SwiftlyCoreB200:
 
         Per facet: ``finish_facet(acc, facet_off1, size, axis=1)``, mask, and
         ``add_to_facet(., subgrid_off0, axis=0, out=facet_acc)`` (api_helper.py:155-179).
-        ``facet_accs[f]``: ``(yN_size, facet_size)``, added to; ``masks1[f]``: float64 device
-        tensor of the facet size or None.
+        ``facet_accs[f]``: ``(yN_size, facet_size)``, added to; or, for every facet, an
+        ``(xM_yN_size, facet_size)`` row ring holding row ``r`` of the column's window at line
+        ``r mod xM_yN_size`` (include/swiftly_b200.h, "Row rings"); ``masks1[f]``: float64
+        device tensor of the facet size or None.
         """
         m, yN = self.xM_yN_size, self.yN_size
 
@@ -779,8 +784,9 @@ class SwiftlyCoreB200:
                 raise ValueError(f"accumulator has shape {tuple(t.shape)}, expected {(m, yN)}!")
 
         def chk_f(t):
-            if t.shape[0] != yN:
-                raise ValueError(f"facet accumulator has {t.shape[0]} rows, expected {yN}!")
+            if t.shape[0] not in (yN, m):
+                raise ValueError(f"facet accumulator has {t.shape[0]} rows, expected {yN} "
+                                 f"(or a ring of {m})!")
 
         keep = []
         for lo in range(0, len(accs), 64):

@@ -266,14 +266,17 @@ static int extract_columns_impl(const swiftly_b200* h, int n_facets,
         return einval("extract_columns: between 1 and " + std::to_string(SW_MAX_COLUMN_FACETS) +
                       " facets per call");
     const int64_t yN = h->yN, m = h->m;
+    // whole prepared facets (yN rows) or row rings (m rows), the same for every facet of a call
+    const int64_t rows = bf_f[0].n_lines == m ? m : yN;
     ExtractColumnsOp op;
     for (int f = 0; f < n_facets; ++f) {
         const swiftly_b200_lines& i = bf_f[f];
         const swiftly_b200_lines& o = out[f];
         if (i.location != SWIFTLY_B200_DEVICE || o.location != SWIFTLY_B200_DEVICE)
             return einval("extract_columns: device arrays only");
-        if (i.n_lines != yN || i.elem_stride != 1 || o.elem_stride != 1)
-            return einval("extract_columns: prepared facets must be yN_size contiguous rows");
+        if (i.n_lines != rows || i.elem_stride != 1 || o.elem_stride != 1)
+            return einval("extract_columns: prepared facets must be yN_size (or, all of them, "
+                          "xM_yN_size ring) contiguous rows");
         if (o.n_lines != m || o.size != yN)
             return einval("extract_columns: output must be xM_yN_size lines of yN_size samples");
         if (i.size > yN - 1) return einval("extract_columns: facet size must be at most yN_size - 1");
@@ -299,6 +302,14 @@ static int extract_columns_impl(const swiftly_b200* h, int n_facets,
     op.scale = 1.0 / (double)yN;
     op.rm_s_m = (int)pmod(sc, m);
     op.rm_base = (int)pmod(yN / 2 - m / 2 + sc, yN);
+    op.rows = (int)rows;
+    if (rows == m) {
+        // row ring: window row r = (rm_base + ((l - s) mod m)) mod yN lives at line r mod m =
+        // (l - (s - rm_base)) mod m (m divides yN), which the kernels' row map yields with
+        // rm_base 0 and the shift s - rm_base -- the kernel code is the same for both forms
+        op.rm_s_m = (int)pmod(op.rm_s_m - op.rm_base, m);
+        op.rm_base = 0;
+    }
     return run_extract_columns(h, op, false, (cudaStream_t)stream);
 }
 
@@ -378,6 +389,8 @@ extern "C" int swiftly_b200_fold_column(const swiftly_b200* h, int n_facets,
         return einval("fold_column: between 1 and " + std::to_string(SW_MAX_COLUMN_FACETS) +
                       " facets per call");
     const int64_t yN = h->yN, m = h->m;
+    // whole facet accumulators (yN rows) or row rings (m rows), the same for every facet
+    const int64_t rows = facet_accs[0].n_lines == m ? m : yN;
     FoldColumnOp op;
     for (int f = 0; f < n_facets; ++f) {
         const swiftly_b200_lines& i = accs[f];
@@ -386,8 +399,9 @@ extern "C" int swiftly_b200_fold_column(const swiftly_b200* h, int n_facets,
             return einval("fold_column: device arrays only");
         if (i.n_lines != m || i.size != yN || i.elem_stride != 1)
             return einval("fold_column: column accumulators must be xM_yN_size lines of yN_size");
-        if (o.n_lines != yN || o.elem_stride != 1 || o.size > yN - 1)
-            return einval("fold_column: facet accumulators must be yN_size lines of facet size");
+        if (o.n_lines != rows || o.elem_stride != 1 || o.size > yN - 1)
+            return einval("fold_column: facet accumulators must be yN_size (or, all of them, "
+                          "xM_yN_size ring) lines of facet size");
         FoldFacet& F = op.fac[f];
         F.in = (const cplx*)i.data;
         F.out = (cplx*)o.data;
@@ -410,5 +424,9 @@ extern "C" int swiftly_b200_fold_column(const swiftly_b200* h, int n_facets,
     op.lines_per = (int)m;
     op.s0_m = (int)pmod(sc, m);
     op.base0 = (int)pmod(yN / 2 - m / 2 + sc, yN);
+    if (rows == m) {  // row ring: line r mod m of window row r, as in extract_columns_impl
+        op.s0_m = (int)pmod(op.s0_m - op.base0, m);
+        op.base0 = 0;
+    }
     return run_fold_column(h, op, false, (cudaStream_t)stream);
 }

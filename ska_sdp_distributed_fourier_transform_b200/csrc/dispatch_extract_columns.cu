@@ -35,7 +35,7 @@ static int launch_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op,
         const int boxes = (max_fs / 8 + k.box_chunks - 1) / k.box_chunks;
         k.in_cap = boxes * k.box_chunks * 8;
         for (int f = 0; f < n_facets && k.swizzled; ++f)
-            if (!make_row_map(&maps.in_map[f], op.fac[f].in, op.fac[f].in_ls, op.n, op.fac[f].fs,
+            if (!make_row_map(&maps.in_map[f], op.fac[f].in, op.fac[f].in_ls, op.rows, op.fac[f].fs,
                               k.box_chunks))
                 k.swizzled = 0;
         if (!k.swizzled) k.in_cap = (max_fs + 1) & ~1;
@@ -108,7 +108,7 @@ static int launch_extract_tma4(const swiftly_b200* h, const ExtractColumnsOp& op
         const int boxes = (max_fs / 8 + k.box_chunks - 1) / k.box_chunks;
         k.in_cap = boxes * k.box_chunks * 8;
         for (int f = 0; f < n_facets && k.swizzled; ++f)
-            if (!make_row_map(&maps.in_map[f], op.fac[f].in, op.fac[f].in_ls, op.n, op.fac[f].fs,
+            if (!make_row_map(&maps.in_map[f], op.fac[f].in, op.fac[f].in_ls, op.rows, op.fac[f].fs,
                               k.box_chunks))
                 k.swizzled = 0;
         if (!k.swizzled) k.in_cap = (max_fs + 1) & ~1;

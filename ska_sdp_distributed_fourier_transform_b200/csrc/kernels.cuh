@@ -166,6 +166,7 @@ struct ExtractColumnsOp {
     int lines_per;     // m
     double scale;      // 1 / yN
     int rm_s_m, rm_base;  // row map: input row = (rm_base + ((l - rm_s_m) mod m)) mod yN
+    int rows;  // (host side) rows of every bf_f: yN, or m for row rings (the TMA row maps)
     SW_HD cplx load(int64_t line, int q) const {
         const int f = (int)(line / lines_per);
         const int l = (int)(line - (int64_t)f * lines_per);
