@@ -208,6 +208,21 @@ int swiftly_b200_extract_columns_windowed(const swiftly_b200* plan, int n_facets
                                           const swiftly_b200_lines* bf_f,
                                           const swiftly_b200_lines* out, int64_t subgrid_off0,
                                           const int64_t* facet_off1, void* stream);
+/* The two finished subgrids of a Hermitian pair (real image: G(-u, -v) = conj(G(u, v))) from
+ * ONE unmasked source, finish_subgrid (core.py:287-325) with api_helper.py:107-111's masks:
+ *   out[r, c]    = mask0[r] * mask1[c] * src[r, c]
+ *   mirror[r, c] = mirror_mask0[r] * mirror_mask1[c] * conj(src[2h - r, 2h - c])
+ * for r, c < sz, h = sz // 2.  src: the subgrid at (off0, off1) of size 2h + 1 (or larger:
+ * only the first 2h + 1 lines and samples are read), lines = rows; out: the subgrid of size sz
+ * at (off0, off1); mirror: the subgrid of size sz at (-off0, -off1).  out and mirror are sz x sz
+ * (overwritten), any line and element strides; every mask may be NULL (all ones), else sz
+ * device doubles.  Device arrays only.  SWIFTLY_B200_EINVAL when src is smaller than 2h + 1 in
+ * either dimension, out and mirror are not both sz x sz, or an array is on the host. */
+int swiftly_b200_mirror_subgrid(const swiftly_b200* plan, const swiftly_b200_lines* src,
+                                const swiftly_b200_lines* out, const swiftly_b200_lines* mirror,
+                                const double* mask0, const double* mask1,
+                                const double* mirror_mask0, const double* mirror_mask1,
+                                void* stream);
 /* ---- fused backward path (device memory only) --------------------------------------- */
 /* One subgrid into the column accumulators of n_facets (<= 64) facets in ONE launch: per
  * facet `extract_from_subgrid(block, facet_off1, axis=1)` followed by `accumulate_column` =

@@ -530,6 +530,54 @@ def _device_mask(mask, device):
     return torch.from_numpy(numpy.ascontiguousarray(arr)).to(device)
 
 
+def _real_facet(idx, data):
+    """``data`` resolved, after checking that it is real-valued (a real floating dtype)."""
+    data = _resolve(data)
+    if isinstance(data, torch.Tensor):
+        real = data.is_floating_point()
+    else:
+        data = numpy.asarray(data)
+        real = data.dtype.kind == "f"
+    if not real:
+        raise ValueError(f"real_image=True: facet {idx} has dtype {data.dtype}, expected a real "
+                         "floating dtype")
+    return data
+
+
+def mirror_pairs(subgrid_configs, N, xM):
+    """How the real-image forward transform covers ``subgrid_configs``: a list of
+    ``(i, j)`` in the order of the sources ``i``, where ``j`` is the index of the config whose
+    subgrid is mirrored from source ``i``, or None when ``i`` is computed alone.
+
+    Configs pair greedily in list order: config ``i`` pairs with the first unpaired later config
+    of the same size at offsets ``(-off0 mod N, -off1 mod N)``, provided the source size
+    ``2 * (size // 2) + 1`` fits ``xM``.  Self-mirrored configs (``2 * off = 0 mod N`` on both
+    axes) stay unpaired.
+    """
+    def key(sg, sign=1):
+        return (sg.size, (sign * sg.off0) % N, (sign * sg.off1) % N)
+
+    later = collections.defaultdict(collections.deque)  # key -> indices, in list order
+    for idx, sg in enumerate(subgrid_configs):
+        later[key(sg)].append(idx)
+    paired = set()
+    plan = []
+    for i, sg in enumerate(subgrid_configs):
+        if i in paired:
+            continue
+        j = None
+        mkey = key(sg, -1)
+        if mkey != key(sg) and 2 * (sg.size // 2) + 1 <= xM:
+            queue = later[mkey]
+            while queue and (queue[0] <= i or queue[0] in paired):
+                queue.popleft()
+            if queue:
+                j = queue.popleft()
+                paired.add(j)
+        plan.append((i, j))
+    return plan
+
+
 # ---------------------------------------------------------------------- forward
 class SwiftlyForward:
     """Facet -> subgrid streaming transform on one GPU.
@@ -550,11 +598,16 @@ class SwiftlyForward:
         (:func:`device_tier_bytes`), the prepared facets live in pinned host memory and
         each subgrid column brings only its ``m``-row window of them to the device (the
         host tier); the subgrids are the same bits either way
+    :param real_image: the facets are real-valued (numpy arrays or tensors of a real floating
+        dtype; ``ValueError`` otherwise).  The grid is then Hermitian, and
+        :meth:`iter_subgrid_tasks` computes one subgrid of each pair at ``(off0, off1)`` /
+        ``(-off0, -off1)`` and mirrors the other (:func:`mirror_pairs`).  Needs the fused
+        kernels (``NotImplementedError`` otherwise).  :meth:`get_subgrid_task` is unchanged
     """
 
     # pylint: disable=too-many-arguments,too-many-instance-attributes
     def __init__(self, swiftly_config, facet_tasks, lru_forward=1, queue_size=20, client=None,
-                 bf_f_buffers=None, device_budget=None):
+                 bf_f_buffers=None, device_budget=None, real_image=False):
         self.config = swiftly_config
         self.facet_tasks = list(facet_tasks)
         self.core = swiftly_config.core
@@ -570,11 +623,16 @@ class SwiftlyForward:
         for idx, (cfg, _) in enumerate(self.facet_tasks):
             rows.setdefault(cfg.off0, []).append(idx)
         self._rows = list(rows.items())
-        self._strips = None
-        self._prep0 = None
-        self._prep1 = None
+        self._sizes = collections.OrderedDict()  # subgrid size -> strips, prepared K3 / K4
         self._masks = {}
         self._fused = bool(getattr(self.core, "fused_forward_supported", lambda: False)())
+        self.real_image = bool(real_image)
+        if self.real_image:
+            if not self._fused:
+                raise NotImplementedError(
+                    "real_image=True needs the fused forward kernels, which this core lacks")
+            self.facet_tasks = [(cfg, _real_facet(idx, data))
+                                for idx, (cfg, data) in enumerate(self.facet_tasks)]
         self.host_tier = self._fused and self._select_host_tier(device_budget)
         self.arena = None
         self._rings = None
@@ -716,34 +774,50 @@ class SwiftlyForward:
                 core, contribs, [cfg for cfg, _ in self.facet_tasks], sg
             )
         m = core.xM_yN_size
-        shape = (len(self._rows), m, sg.size)
-        if self._strips is None or tuple(self._strips.shape) != shape:
-            # stored TRANSPOSED -- (row, xA, m), contribution index contiguous -- so that the
-            # axis-0 kernel reads unit-stride lines; the axis-1 kernel's finished lines are
-            # scattered into this layout by the TMA engine (bulk tensor stores)
-            self._strips = torch.empty((shape[0], shape[2], shape[1]), dtype=torch.complex128,
-                                       device=self.device).transpose(1, 2)
-            self._prep0 = None
+        st = self._size_state(sg.size)
+        strips = st["strips"]
         mask0 = self._mask(sg, 0)
         mask1 = self._mask(sg, 1)
         # the argument blocks are built once per subgrid column (axis 1) / once per transform
-        # (axis 0) and reused: per subgrid only offsets, masks and the output pointer change
+        # (axis 0) and subgrid size, and reused: per subgrid only offsets, masks and the output
+        # pointer change
         key = id(NMBF_BFs)
-        if self._prep1 is None or self._prep1[0] != key or self._prep1[1] != sg.size:
-            groups = [[(NMBF_BFs[j], self.facet_tasks[j][0].off1) for j in members]
+        if st["prep1"] is None or st["prep1"][0] != key:
+            for other in self._sizes.values():  # no block keeps an earlier column alive
+                if other["prep1"] is not None and other["prep1"][0] != key:
+                    other["prep1"] = None
+            groups =[[(NMBF_BFs[j], self.facet_tasks[j][0].off1) for j in members]
                       for _, members in self._rows]
-            self._prep1 = (key, sg.size, core.prepare_sum_finish(
-                groups, 1, m, sg.size, (self._strips.stride(1), self._strips.stride(2))), NMBF_BFs)
+            st["prep1"] = (key, core.prepare_sum_finish(
+                groups, 1, m, sg.size, (strips.stride(1), strips.stride(2))), NMBF_BFs)
         nrows = len(self._rows)
-        self._prep1[2].launch([sg.off1] * nrows, [mask1] * nrows, out=self._strips,
-                              out_group_stride=self._strips.stride(0))
+        st["prep1"][1].launch([sg.off1] * nrows, [mask1] * nrows, out=strips,
+                              out_group_stride=strips.stride(0))
         out = torch.empty((sg.size, sg.size), dtype=torch.complex128, device=self.device)
-        if self._prep0 is None or self._prep0[0] != sg.size:
-            sources = [[(self._strips[r], off0) for r, (off0, _) in enumerate(self._rows)]]
-            self._prep0 = (sg.size, core.prepare_sum_finish(
-                sources, 0, sg.size, sg.size, (out.stride(1), out.stride(0))))
-        self._prep0[1].launch([sg.off0], [mask0], out=out)
+        if st["prep0"] is None:
+            sources = [[(strips[r], off0) for r, (off0, _) in enumerate(self._rows)]]
+            st["prep0"] = core.prepare_sum_finish(
+                sources, 0, sg.size, sg.size, (out.stride(1), out.stride(0)))
+        st["prep0"].launch([sg.off0], [mask0], out=out)
         return out
+
+    def _size_state(self, size):
+        """Subgrid strips and prepared K3 / K4 blocks of one subgrid size.  The two sizes used
+        last are kept: the real-image mode alternates a column's source size ``S`` and its
+        subgrid size when the column holds self-mirrored subgrids."""
+        st = self._sizes.get(size)
+        if st is None:
+            # strips stored TRANSPOSED -- (row, xA, m), contribution index contiguous -- so that
+            # the axis-0 kernel reads unit-stride lines; the axis-1 kernel's finished lines are
+            # scattered into this layout by the TMA engine (bulk tensor stores)
+            strips = torch.empty((len(self._rows), size, self.core.xM_yN_size),
+                                 dtype=torch.complex128, device=self.device).transpose(1, 2)
+            st = {"strips": strips, "prep1": None, "prep0": None}
+            if len(self._sizes) >= 2:
+                self._sizes.popitem(last=False)
+            self._sizes[size] = st
+        self._sizes.move_to_end(size)
+        return st
 
     def _mask(self, sg, axis):
         """Device mask of a subgrid along ``axis`` (None when absent or all ones), cached by
@@ -761,6 +835,40 @@ class SwiftlyForward:
         task = DeviceTask(self._gen_subgrid(subgrid_config, NMBF_BFs))
         self.task_queue.process([task])
         return task
+
+    def iter_subgrid_tasks(self, subgrid_configs):
+        """Enqueue every subgrid of ``subgrid_configs``; yields ``(index, task)`` once per config.
+
+        Default: :meth:`get_subgrid_task` in list order.  With ``real_image``, configs pair as
+        :func:`mirror_pairs` says.  A pair's source is computed once, without masks, at the odd
+        size ``S = 2 * (size // 2) + 1`` (K2 for its column, K3 and K4 at ``S``); one
+        ``mirror_subgrid`` launch then writes both subgrids with their own masks.  The source's
+        task is yielded first, its mirror's right after.  Unpaired configs run
+        :meth:`get_subgrid_task`.
+        """
+        configs = list(subgrid_configs)
+        if not self.real_image:
+            for i, sg in enumerate(configs):
+                yield i, self.get_subgrid_task(sg)
+            return
+        for i, j in mirror_pairs(configs, self.config.image_size,
+                                 self.config.internal_subgrid_size):
+            if j is None:
+                yield i, self.get_subgrid_task(configs[i])
+                continue
+            sg, mg = configs[i], configs[j]
+            BF_Fs = self._get_BF_Fs()
+            NMBF_BFs = self.get_NMBF_BFs_off0(sg.off0, BF_Fs)
+            size = 2 * (sg.size // 2) + 1
+            src = self._gen_subgrid(SubgridConfig(sg.off0, sg.off1, size), NMBF_BFs)
+            out, mirror = self.core.mirror_subgrid(
+                src, sg.size, masks=(self._mask(sg, 0), self._mask(sg, 1)),
+                mirror_masks=(self._mask(mg, 0), self._mask(mg, 1)))
+            del src
+            tasks = [DeviceTask(out), DeviceTask(mirror)]
+            self.task_queue.process(tasks)
+            yield i, tasks[0]
+            yield j, tasks[1]
 
 
 # ---------------------------------------------------------------------- backward

@@ -654,6 +654,50 @@ class SwiftlyCoreB200:
         _lib.check(self._lib, rc)
         return out
 
+    def mirror_subgrid(self, src, sz, out=None, mirror=None, masks=None, mirror_masks=None):
+        """The two finished subgrids of a Hermitian pair (real image) from ONE unmasked source.
+
+        ``src``: the subgrid at ``(off0, off1)`` of size ``S = 2 * (sz // 2) + 1`` or larger (only
+        the first ``S x S`` samples are read), e.g. ``sum_finish_axis`` along both axes at size
+        ``S`` without masks.  Returns ``(out, mirror)``, both ``(sz, sz)``:
+        ``out[r, c] = m0[r] * m1[c] * src[r, c]`` is the subgrid of size ``sz`` at
+        ``(off0, off1)``; ``mirror[r, c] = n0[r] * n1[c] * conj(src[2h - r, 2h - c])``,
+        ``h = sz // 2``, the one at ``(-off0, -off1)``.  ``masks`` / ``mirror_masks``: None or
+        ``(mask0, mask1)``, each None or a float64 device tensor of ``sz`` samples.  ``out`` /
+        ``mirror`` may be given (any strides, e.g. views into larger arrays); device tensors only.
+        """
+        self._check_tensor(src)
+        if src.dtype != torch.complex128 or src.dim() != 2:
+            raise ValueError("mirror_subgrid needs a 2-D complex128 device tensor")
+        shape = (int(sz), int(sz))
+        outs = []
+        for t in (out, mirror):
+            if t is None:
+                t = torch.empty(shape, dtype=torch.complex128, device=src.device)
+            self._check_tensor(t)
+            if t.dtype != torch.complex128 or tuple(t.shape) != shape:
+                raise ValueError(f"Output array has shape {tuple(t.shape)}, expected {shape}!")
+            outs.append(t)
+        keep = []
+        ptrs = []
+        for pair in (masks, mirror_masks):
+            for mk in (None, None) if pair is None else pair:
+                if mk is None:
+                    ptrs.append(None)
+                    continue
+                mk = mk.to(torch.float64).contiguous()
+                self._check_tensor(mk)
+                if mk.numel() != shape[0]:
+                    raise ValueError("mask must have the subgrid size")
+                keep.append(mk)
+                ptrs.append(mk.data_ptr())
+        din, dout, dmir = (self._describe(t, 1) for t in (src, outs[0], outs[1]))
+        rc = self._lib.swiftly_b200_mirror_subgrid(
+            self._plan, ctypes.byref(din), ctypes.byref(dout), ctypes.byref(dmir), *ptrs,
+            self._stream(src))
+        _lib.check(self._lib, rc)
+        return outs[0], outs[1]
+
     def release_scratch(self):
         """Give the plan's scratch buffers (2 GiB after stage 1 at N = 65536) back to the device."""
         self._lib.swiftly_b200_release_scratch(self._plan)

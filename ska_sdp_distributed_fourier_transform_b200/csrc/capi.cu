@@ -210,7 +210,8 @@ extern "C" void swiftly_b200_debug_sg_variant(swiftly_b200* h, int variant) {
 // 4 LineKernel, 5 SplitLineKernel, 6 SplitFKernel, 7 WindowCopyKernel; the TMA-staged
 // extract_columns kernels: 8 ExtractColumnsTmaKernel<yN, false>, 9 its 2 x yN/2 split,
 // 10 ExtractColumnsTma4Kernel, 11 ExtractColumnsTmaDifKernel, 12 / 13 / 14
-// ExtractColumnsParkKernel MODE 0 / 1 / 2, 15 ExtractColumnsParkSkewKernel); out[1]: lines per
+// ExtractColumnsParkKernel MODE 0 / 1 / 2, 15 ExtractColumnsParkSkewKernel; 16
+// MirrorSubgridKernel, with 0 in out[1] and out[2]); out[1]: lines per
 // CTA (1 .. 4), F (5, 6: 2 for SplitLineKernel), 0 (7), or for 8 .. 15 the 128-byte chunks per
 // tensor load when the rows are staged swizzled and 0 when they are staged by linear bulk
 // copies; out[2]: output path of the fused kernels (0 direct stores, 1 TMA with one tensor map,

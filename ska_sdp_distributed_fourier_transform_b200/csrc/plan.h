@@ -59,7 +59,8 @@ enum {
     LAUNCH_K2_PARK_DIF = 12,   // ExtractColumnsParkKernel<yN / 4, 0>: facets of at most yN / 2
     LAUNCH_K2_PARK_DIF2 = 13,  // ExtractColumnsParkKernel<yN / 4, 1>: longer facets
     LAUNCH_K2_PARK_DIT = 14,   // ExtractColumnsParkKernel<yN / 4, 2>
-    LAUNCH_K2_PARK_SKEW = 15   // ExtractColumnsParkSkewKernel<yN / 4>
+    LAUNCH_K2_PARK_SKEW = 15,  // ExtractColumnsParkSkewKernel<yN / 4>
+    LAUNCH_MIRROR = 16         // MirrorSubgridKernel (dispatch_mirror_subgrid.cu): 0, 0
 };
 
 // records the form of a launch for swiftly_b200_debug_last_launch (one host-side store)
