@@ -145,6 +145,7 @@ extern "C" int swiftly_b200_create(double W, int64_t N, int64_t xM, int64_t yN, 
     h->sg_variant = 0;
     h->max_blocks = 0;
     for (int i = 0; i < 4; ++i) h->last_launch[i] = 0;
+    h->last_cluster = 1;
     cudaError_t e = cudaMalloc((void**)&h->d_Fb, sizeof(double) * (size_t)(yN > 1 ? yN - 1 : 1));
     if (e == cudaSuccess) e = cudaMalloc((void**)&h->d_Fn, sizeof(double) * (size_t)h->m);
     if (e == cudaSuccess)
@@ -221,6 +222,12 @@ extern "C" void swiftly_b200_debug_sg_variant(swiftly_b200* h, int variant) {
 extern "C" void swiftly_b200_debug_last_launch(const swiftly_b200* h, int* out) {
     if (h && out)
         for (int i = 0; i < 4; ++i) out[i] = h->last_launch[i];
+}
+
+// test hook: CTAs per cluster of the last launch recorded by swiftly_b200_debug_last_launch (2
+// when the 4 x Q form of extract_columns ran on two-CTA clusters, else 1)
+extern "C" int swiftly_b200_debug_last_cluster(const swiftly_b200* h) {
+    return h ? h->last_cluster : 0;
 }
 
 // ------------------------------------------------------------------ host staging

@@ -15,6 +15,7 @@
 
 #if defined(SWIFTLY_EMU)
 #include "emu_runtime.h"
+#include "emu_cluster.h"
 #else
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -230,6 +231,61 @@ struct DeviceCtx {
     // region out so that the 32 threads of a warp touch 512 contiguous bytes.
     __device__ __forceinline__ void park_st(cplx* p, cplx v) const { __stcg(p, v); }
     __device__ __forceinline__ cplx park_ld(const cplx* p) const { return __ldcg(p); }
+    // ---- thread block clusters (kernels launched with a cluster dimension) ----
+    // rank of this CTA in its cluster
+    __device__ __forceinline__ int cluster_rank() const {
+        uint32_t r;
+        asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+        return (int)r;
+    }
+    // barrier over every thread of the cluster; orders shared-memory accesses across its CTAs
+    __device__ __forceinline__ void cluster_sync() const {
+        asm volatile("barrier.cluster.arrive.release.aligned;\n"
+                     "barrier.cluster.wait.acquire.aligned;" ::: "memory");
+    }
+    // the shared-memory word of CTA `rank` of the cluster at the offset of the local `p`
+    __device__ __forceinline__ static uint32_t peer_addr(const void* p, int rank) {
+        uint32_t a;
+        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;"
+                     : "=r"(a) : "r"((uint32_t)__cvta_generic_to_shared(p)), "r"(rank));
+        return a;
+    }
+    // store into the shared memory of CTA `rank` (distributed shared memory)
+    __device__ __forceinline__ void peer_st(cplx* p, int rank, cplx v) const {
+        asm volatile("st.shared::cluster.v2.f64 [%0], {%1, %2};"
+                     ::"r"(peer_addr(p, rank)), "d"(v.x), "d"(v.y) : "memory");
+    }
+    // atomic add to a counter in the shared memory of CTA `rank`; returns the previous value
+    __device__ __forceinline__ int peer_atomic_add(int* p, int rank, int v) const {
+        int prev;
+        asm volatile("atom.relaxed.cluster.shared::cluster.add.u32 %0, [%1], %2;"
+                     : "=r"(prev) : "r"(peer_addr(p, rank)), "r"(v) : "memory");
+        return prev;
+    }
+    // tx_expect on the bulk-copy barrier of CTA `rank` at the offset of the local `bar`
+    __device__ __forceinline__ void tx_expect_peer(uint64_t* bar, int rank, uint32_t bytes) const {
+        asm volatile("mbarrier.arrive.expect_tx.shared::cluster.b64 _, [%0], %1;"
+                     ::"r"(peer_addr(bar, rank)), "r"(bytes) : "memory");
+    }
+    // tensor_load / tx_copy delivered to the same offsets in every CTA of `mask`: the data to
+    // `smem_dst`, the completion to the barrier at `bar` of each of them
+    __device__ __forceinline__ void tensor_load_mc(void* smem_dst, const void* map, int c1, int c2,
+                                                   uint64_t* bar, uint16_t mask) const {
+        asm volatile(
+            "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes"
+            ".multicast::cluster [%0], [%1, {%2, %3, %4, %5}], [%6], %7;"
+            ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(map), "r"(0), "r"(c1),
+              "r"(c2), "r"(0), "r"((uint32_t)__cvta_generic_to_shared(bar)), "h"(mask)
+            : "memory");
+    }
+    __device__ __forceinline__ void tx_copy_mc(void* smem_dst, const void* gmem_src, uint32_t bytes,
+                                               uint64_t* bar, uint16_t mask) const {
+        asm volatile(
+            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+            " [%0], [%1], %2, [%3], %4;"
+            ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gmem_src), "r"(bytes),
+              "r"((uint32_t)__cvta_generic_to_shared(bar)), "h"(mask) : "memory");
+    }
 };
 
 extern __shared__ __align__(1024) char swiftly_dyn_smem[];
@@ -306,6 +362,34 @@ inline cudaError_t launch_body_maps(const Body& body, const typename Body::Maps&
     }
     kernel_entry_maps<Body><<<grid, Body::THREADS, smem_bytes, stream>>>(body, maps);
     return cudaGetLastError();
+}
+
+// kernel_entry_maps launched in clusters of Body::CLUSTER consecutive CTAs (grid a multiple of
+// it).  Without a stream, only asks how many such clusters the device can hold at once
+// (*clusters; 0: a cluster cannot be placed at all).
+template <class Body>
+inline cudaError_t launch_body_maps_cluster(const Body& body, const typename Body::Maps& maps,
+                                            int grid, size_t smem_bytes, cudaStream_t stream,
+                                            int* clusters) {
+    cudaError_t e = cudaFuncSetAttribute(kernel_entry_maps<Body>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem_bytes);
+    if (e != cudaSuccess) return e;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = Body::CLUSTER;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid > 0 ? grid : Body::CLUSTER);
+    cfg.blockDim = dim3(Body::THREADS);
+    cfg.dynamicSmemBytes = smem_bytes;
+    cfg.stream = stream;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    if (clusters) return cudaOccupancyMaxActiveClusters(clusters, kernel_entry_maps<Body>, &cfg);
+    if (grid <= 0) return cudaSuccess;
+    return cudaLaunchKernelEx(&cfg, kernel_entry_maps<Body>, body, maps);
 }
 #endif
 

@@ -83,16 +83,13 @@ struct K2Code<ExtractColumnsParkSkewKernel<Q>> {
     static const int value = LAUNCH_K2_PARK_SKEW;
 };
 
-// 4 x Q split with two thread groups (extract_tma.cuh)
-template <int Q, class K>
-static int launch_extract_tma4(const swiftly_b200* h, const ExtractColumnsOp& op, int max_fs,
-                               cudaStream_t s, int scratch_lines) {
-    K k;
-    static thread_local typename K::Maps maps;
-    k.op = op;
-    k.tw = twiddles(h, Q);
-    k.twf = twiddles_full(h, 4 * Q);
-    if (!k.tw || !k.twf) return SWIFTLY_B200_ECUDA;
+// staging of the 4 x Q kernels: swizzled tensor loads when every facet row is whole 128-byte
+// chunks and the buffer in whole boxes fits (sg_variant 6: linear), else linear bulk copies.
+// Fills k.in_cap / swizzled / box_chunks and the row maps; returns the shared memory of a CTA,
+// 0 when even the linear staging does not fit
+template <class K>
+static size_t stage_extract_tma4(const swiftly_b200* h, const ExtractColumnsOp& op, int max_fs,
+                                 K& k, typename K::Maps& maps) {
     const int n_facets = (int)(op.g.n_lines / op.lines_per);
     k.in_cap = (max_fs + 1) & ~1;
     k.swizzled = h->sg_variant != 6 ? 1 : 0;
@@ -118,7 +115,21 @@ static int launch_extract_tma4(const swiftly_b200* h, const ExtractColumnsOp& op
         k.in_cap = (max_fs + 1) & ~1;
     }
     const size_t smem = K::smem_bytes(k.in_cap);
-    if (smem > (size_t)227 * 1024) return -1;
+    return smem > (size_t)227 * 1024 ? 0 : smem;
+}
+
+// 4 x Q split with two thread groups (extract_tma.cuh)
+template <int Q, class K>
+static int launch_extract_tma4(const swiftly_b200* h, const ExtractColumnsOp& op, int max_fs,
+                               cudaStream_t s, int scratch_lines) {
+    K k;
+    static thread_local typename K::Maps maps;
+    k.op = op;
+    k.tw = twiddles(h, Q);
+    k.twf = twiddles_full(h, 4 * Q);
+    if (!k.tw || !k.twf) return SWIFTLY_B200_ECUDA;
+    const size_t smem = stage_extract_tma4(h, op, max_fs, k, maps);
+    if (!smem) return -1;
     int per_sm = (int)((size_t)227 * 1024 / smem);
     if (per_sm > 512 / K::THREADS) per_sm = 512 / K::THREADS;  // 128 registers per thread
     if (per_sm < 1) per_sm = 1;
@@ -134,6 +145,35 @@ static int launch_extract_tma4(const swiftly_b200* h, const ExtractColumnsOp& op
     cudaError_t e = launch_body_maps(k, maps, (int)blocks, smem, s);
     return e == cudaSuccess ? SWIFTLY_B200_OK
                             : cuda_fail(e, "extract_columns (TMA, 4-way split) kernel launch");
+}
+
+// 4 x Q split on two-CTA clusters (extract_tma.cuh): the grid of the single-CTA form (one CTA per
+// SM, at most one per line, at most max_blocks), its CTAs paired.  Returns -1 when that grid is
+// odd or the device cannot hold all its clusters at once (then the single-CTA form runs on it).
+template <int Q>
+static int launch_extract_cluster(const swiftly_b200* h, const ExtractColumnsOp& op, int max_fs,
+                                  cudaStream_t s) {
+    typedef ExtractColumnsClusterKernel<Q> K;
+    K k;
+    static thread_local typename K::Maps maps;
+    k.op = op;
+    k.tw = twiddles(h, Q);
+    k.twf = twiddles_full(h, 4 * Q);
+    if (!k.tw || !k.twf) return SWIFTLY_B200_ECUDA;
+    const size_t smem = stage_extract_tma4(h, op, max_fs, k, maps);
+    if (!smem) return -1;
+    int64_t blocks = NUM_SMS;  // one CTA of 512 threads per SM, as launch_extract_tma4
+    if (blocks > op.g.n_lines) blocks = op.g.n_lines;
+    if (h->max_blocks > 0 && blocks > h->max_blocks) blocks = h->max_blocks;
+    if (blocks % K::CLUSTER != 0) return -1;
+    int clusters = 0;
+    cudaError_t e = launch_body_maps_cluster(k, maps, 0, smem, s, &clusters);
+    if (e != cudaSuccess) return cuda_fail(e, "extract_columns (TMA, cluster) occupancy query");
+    if (clusters < blocks / K::CLUSTER) return -1;
+    note_launch(h, LAUNCH_K2_TMA4, k.swizzled ? k.box_chunks : 0, k.in_cap, (int)blocks, K::CLUSTER);
+    e = launch_body_maps_cluster(k, maps, (int)blocks, smem, s, nullptr);
+    return e == cudaSuccess ? SWIFTLY_B200_OK
+                            : cuda_fail(e, "extract_columns (TMA, cluster) kernel launch");
 }
 
 // K2 with intermediate results parked in L2-resident scratch (extract_park.cuh): PARK samples
@@ -176,14 +216,17 @@ static int try_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op, cu
         if (h->sg_variant != 7 && h->force_split != 1) {
             switch (n) {
                 case 16384: {
-                    // DEFAULT: the 4 x Q form with a CTA-wide combine through an L2 scratch
-                    // (extract_tma.cuh).  The forms that park intermediate results per thread in
+                    // DEFAULT: the 4 x Q form on two-CTA clusters that combine through
+                    // distributed shared memory (extract_tma.cuh); 26: the same on one CTA with
+                    // the combine through an L2 scratch, which also runs when the grid cannot be
+                    // paired.  The forms that park intermediate results per thread in
                     // L2-resident scratch (extract_park.cuh) stay selectable: 19 = DIT within and
                     // across the groups, store phases half a line apart; 18 = the same without the
                     // skew; 17 = DIF across the groups, 32-byte pair stores; 15 = two independent
                     // groups, 16-byte stores at 32-byte stride.  Measured on an H100 80GB HBM3
-                    // (700 W), 8 facets of pre-windowed rows (tools/quick_k2.py): default 2.23 ms,
-                    // 17: 3.14, 18: 3.78, 19: 4.01, 15: 3.98.
+                    // (700 W), 8 facets of pre-windowed rows (tools/quick_k2.py): default 1.56 ms,
+                    // 26: 2.19 (2.23 in an earlier session, with 17: 3.14, 18: 3.78, 19: 4.01,
+                    // 15: 3.98).
                     if (h->sg_variant == 17 && pair_store_ok(op, n_facets)) {
                         int rc = max_fs <= n / 2
                             ? launch_extract_park<4096, ExtractColumnsParkKernel<4096, 0>>(h, op, max_fs, s)
@@ -196,6 +239,10 @@ static int try_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op, cu
                     }
                     if (h->sg_variant == 19) {
                         int rc = launch_extract_park<4096, ExtractColumnsParkSkewKernel<4096>>(h, op, max_fs, s);
+                        if (rc != -1) return rc;
+                    }
+                    if (h->sg_variant != 15 && h->sg_variant != 26) {
+                        int rc = launch_extract_cluster<4096>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
                     int rc = h->sg_variant != 15
@@ -220,6 +267,11 @@ static int try_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op, cu
                     }
                     if (h->force_split == 6) {
                         int rc = launch_extract_park<128, ExtractColumnsParkSkewKernel<128>>(h, op, max_fs, s);
+                        if (rc != -1) return rc;
+                    }
+                    // force_split 2: as the default at yN = 16384, 7: as sg_variant 26
+                    if (h->force_split == 2) {
+                        int rc = launch_extract_cluster<128>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
                     int rc = h->force_split != 3

@@ -26,27 +26,46 @@ namespace swiftly {
 // 128-byte swizzle when the rows are whole 128-byte chunks (tensor_map.cu make_row_map; a box
 // that sticks out of the row is zero filled and still counts in full), else 1-D bulk copies in
 // pieces of at most 64 KiB.  Shared by all TMA-staged K2 kernels.
-template <class Maps, class Ctx>
+// PAIR: the row goes to the same offsets in both CTAs of a two-CTA cluster (multicast); the
+// issuing thread, of either CTA, arms both CTAs' barriers.
+template <class Maps, bool PAIR = false, class Ctx>
 SW_HD void k2_issue_row(const Ctx& ctx, const ExtractColumnsOp& op, int swizzled, int box_chunks,
                         cplx* in, uint64_t* bar, int64_t line) {
     const int f = (int)(line / op.lines_per);
     const int l = (int)(line - (int64_t)f * op.lines_per);
     const ColumnFacet& F = op.fac[f];
     const int64_t row = wrap_add(op.rm_base, wrap_sub(l, op.rm_s_m, op.lines_per), op.n);
+    auto expect = [&](uint32_t bytes) {
+        if constexpr (PAIR) {
+            ctx.tx_expect_peer(bar, 0, bytes);
+            ctx.tx_expect_peer(bar, 1, bytes);
+        } else {
+            ctx.tx_expect(bar, bytes);
+        }
+    };
     if (swizzled) {
         const int chunks = F.fs / 8;
         const int boxes = (chunks + box_chunks - 1) / box_chunks;
-        ctx.tx_expect(bar, (uint32_t)boxes * (uint32_t)box_chunks * 128u);
-        for (int c0 = 0; c0 < chunks; c0 += box_chunks)
-            ctx.tensor_load((char*)in + (size_t)c0 * 128, &((const Maps*)ctx.tmaps)->in_map[f], c0,
-                            (int)row, bar);
+        expect((uint32_t)boxes * (uint32_t)box_chunks * 128u);
+        for (int c0 = 0; c0 < chunks; c0 += box_chunks) {
+            const TensorMap4* map = &((const Maps*)ctx.tmaps)->in_map[f];
+            if constexpr (PAIR)
+                ctx.tensor_load_mc((char*)in + (size_t)c0 * 128, map, c0, (int)row, bar, 3);
+            else
+                ctx.tensor_load((char*)in + (size_t)c0 * 128, map, c0, (int)row, bar);
+        }
         return;
     }
     const uint32_t bytes = (uint32_t)F.fs * (uint32_t)sizeof(cplx);
-    ctx.tx_expect(bar, bytes);
+    expect(bytes);
     const char* src = (const char*)(F.in + row * F.in_ls);
-    for (uint32_t o = 0; o < bytes; o += 65536u)
-        ctx.tx_copy((char*)in + o, src + o, bytes - o < 65536u ? bytes - o : 65536u, bar);
+    for (uint32_t o = 0; o < bytes; o += 65536u) {
+        const uint32_t piece = bytes - o < 65536u ? bytes - o : 65536u;
+        if constexpr (PAIR)
+            ctx.tx_copy_mc((char*)in + o, src + o, piece, bar, 3);
+        else
+            ctx.tx_copy((char*)in + o, src + o, piece, bar);
+    }
 }
 
 template <int H, bool SPLIT>
@@ -344,6 +363,186 @@ struct ExtractColumnsTma4Kernel {
                 }
             }
             ctx.sync();  // scratch and exchange buffers are reused by the next line
+        }
+    }
+};
+
+// ---------------------------------------------------------------------------------------
+// yN = 4 Q as above, on a CLUSTER of two CTAs that share every line: no L2 scratch.
+//
+// The row is staged once for both CTAs by multicast loads.  CTA c runs t_c in group 0 and
+// t_(c+2) in group 1, one Q-point transform per group and line; a thread owns the same outputs
+// k = tg + TG i (i < 16) in every sub-transform and keeps half of its t_q[k] in registers.  The
+// radix-4 butterfly over q (bfly4) pairs q with q + 2 first:
+//   P+ = t_0 + t_2,  P- = t_0 - t_2          (CTA 0)
+//   R+ = t_1 + t_3,  R- = i (t_1 - t_3)      (CTA 1)
+//   X_0 = P+ + R+,  X_2 = P+ - R+            (stored by CTA 0)
+//   X_1 = P- + R-,  X_3 = P- - R-            (stored by CTA 1)
+// 1. inside the CTA the groups swap the other half of their t_q through their exchange buffers
+//    (dead after the last pass's reads): group g then holds both operands for i in [8 g, 8 g + 8)
+//    and forms P or R there;
+// 2. CTA 0 writes P-, CTA 1 writes R+ into the partner's exchange buffers (distributed shared
+//    memory, Q samples each way), and after a cluster barrier each CTA finishes two outputs.
+// Same operations in the same order as ExtractColumnsTma4Kernel, so the same bits.  The staging
+// buffer is dead once all four groups of the pair have done their first-pass loads: the last of
+// them to get there issues the next row (counter in CTA 0).
+template <int Q>
+struct ExtractColumnsClusterKernel {
+    static constexpr int DIR = +1;
+    static constexpr int CLUSTER = 2;
+    static constexpr int TG = FftCfg<Q>::T;
+    static constexpr int THREADS = 2 * TG;
+    static constexpr int N = 4 * Q;
+    static constexpr int XBUF = (FftCfg<Q>::PADDED + 1) & ~1;
+    // the half of a group's 16 outputs that changes hands fits its exchange buffer
+    static_assert(8 * TG * 2 <= XBUF, "exchange buffer too small for the combine");
+    static constexpr size_t smem_bytes(int in_cap) {
+        return (size_t)in_cap * sizeof(cplx) + 2 * (size_t)XBUF * sizeof(double) + 32;
+    }
+
+    ExtractColumnsOp op;
+    const cplx* tw;   // compact table of the Q-point plan
+    const cplx* twf;  // exp(-2 pi i t / yN), t < yN / 2
+    int in_cap;
+    int swizzled;
+    int box_chunks;
+    struct Maps {
+        TensorMap4 in_map[SW_MAX_COLUMN_FACETS];
+    };
+
+    SW_HD cplx root(int t) const {  // exp(DIR 2 pi i t / N), 0 <= t < N
+        const bool neg = t >= N / 2;
+        cplx w = ldg_c(twf + (neg ? t - N / 2 : t));
+        if (DIR > 0) w.y = -w.y;
+        return neg ? mk(-w.x, -w.y) : w;
+    }
+
+    template <class Ctx>
+    SW_HD void issue(const Ctx& ctx, cplx* in, uint64_t* bar, int64_t line) const {
+        k2_issue_row<Maps, true>(ctx, op, swizzled, box_chunks, in, bar, line);
+    }
+
+    template <class Ctx>
+    struct GroupSync {
+        const Ctx& ctx;
+        const ExtractColumnsClusterKernel& k;
+        int grp, tg;
+        cplx* in;
+        uint64_t* bar;
+        int* done;  // counter in CTA 0
+        int64_t next_line;
+        bool pending;
+        SW_HD void operator()() {
+            ctx.group_sync(1 + grp, TG);
+            if (pending) {
+                pending = false;
+                if (tg == 0 && (ctx.peer_atomic_add(done, 0, 1) & 3) == 3 &&
+                    next_line < k.op.g.n_lines)
+                    k.issue(ctx, in, bar, next_line);
+            }
+        }
+        SW_HD void pre_store() { ctx.group_sync(1 + grp, TG); }
+    };
+
+    template <class Ctx>
+    SW_HD void operator()(Ctx& ctx) const {
+        cplx* in = (cplx*)ctx.smem;
+        double* xb = (double*)(in + in_cap);
+        uint64_t* bar = (uint64_t*)(xb + 2 * XBUF);
+        int* done = (int*)(bar + 1);
+        const int rank = ctx.cluster_rank();
+        const int cid = ctx.bid / CLUSTER, ncl = ctx.nblocks / CLUSTER;
+        const int grp = ctx.tid / TG;
+        const int tg = ctx.tid % TG;
+        double* sm = xb + (size_t)grp * XBUF;
+        cplx* mine = (cplx*)sm;                        // this group's exchange buffer
+        cplx* other = (cplx*)(xb + (size_t)(1 - grp) * XBUF);
+        constexpr int n = N;  // op.n
+        const int q4 = rank + 2 * grp;
+        const int lo = 8 * grp;  // the outputs i in [lo, lo + 8) are combined by this group
+        if (ctx.tid == 0) {
+            ctx.tx_init(bar);
+            *done = 0;
+        }
+        ctx.cluster_sync();  // both barriers initialised before the first multicast
+        if (rank == 0 && ctx.tid == 0 && cid < op.g.n_lines) issue(ctx, in, bar, cid);
+        uint32_t parity = 0;
+        typedef LastPass<Q> LP;
+        for (int64_t line = cid; line < op.g.n_lines; line += ncl) {
+            const int f = (int)(line / op.lines_per);
+            const int l = (int)(line - (int64_t)f * op.lines_per);
+            const ColumnFacet& F = op.fac[f];
+            const int shift_in = F.shift_in, fs = F.fs;
+            const double* fb = op.fb ? op.fb + F.fb_off : nullptr;
+            cplx* o = F.out + (int64_t)l * F.out_ls;
+            const double scale = op.scale;
+            const bool swz = swizzled != 0;
+            auto sample = [&](int q) {
+                int k = wrap_add(q, shift_in, n);
+                if (k >= fs) return mk(0.0, 0.0);
+                const int ks = swz ? ((k & ~7) | ((k ^ (k >> 3)) & 7)) : k;
+                return fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+            };
+            ctx.tx_wait(bar, parity);
+            parity ^= 1;
+            GroupSync<Ctx> gs{ctx, *this, grp, tg, in, bar, done, line + ncl, true};
+            // t_q[k] of the thread's outputs k = tg + TG i, i = it + ITERS r of the last pass:
+            // group 0 combines i < 8 and keeps those, group 1 the others; the other half goes to
+            // the group's exchange buffer as soon as the group has done its last exchange reads
+            // (GroupSync::pre_store)
+            cplx t[8];
+            {
+                auto ld = [&](int j) { return sample(4 * j + q4); };
+                const cplx step_it = root((q4 * TG) % N), step_r = root((q4 * LP::NS) % N);
+                cplx w_it = mk(1.0, 0.0), w = mk(1.0, 0.0);
+                auto st = [&](int k, cplx v, int it, int r) {
+                    if (r == 0) {
+                        w_it = it == 0 ? root((q4 * k) % N) : cmul(w_it, step_it);
+                        w = w_it;
+                    } else {
+                        w = cmul(w, step_r);
+                    }
+                    const int i = it + LP::ITERS * r;  // (output i - 8 comes before i)
+                    const cplx tq = q4 ? cmul(v, w) : v;
+                    if (i < 8) {
+                        t[i] = tq;
+                    } else {  // outputs i - 8 and i: keep one, pass the other on
+                        const cplx keep = grp ? tq : t[i - 8];
+                        mine[(i - 8) * TG + tg] = grp ? t[i - 8] : tq;
+                        t[i - 8] = keep;
+                    }
+                };
+                line_fft<Q, DIR>(tg, sm, tw, ld, st, gs);
+            }
+            ctx.sync();  // both halves are in the exchange buffers
+            // (a, b) = (t_rank, t_(rank+2)) at output lo + i; CTA 0: P+ / P-, CTA 1: R+ / R-
+            cplx keep[8], send[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const cplx u = other[i * TG + tg];  // the CTA's other q
+                const cplx a = grp ? u : t[i], b = grp ? t[i] : u;
+                const cplx s = cadd(a, b), d = csub(a, b);
+                keep[i] = rank ? mul_i<DIR>(d) : s;  // R- or P+
+                send[i] = rank ? s : d;              // R+ to CTA 0, P- to CTA 1
+            }
+            // trade with the partner CTA once it has read its exchange buffers
+            ctx.cluster_sync();
+#pragma unroll
+            for (int i = 0; i < 8; ++i) ctx.peer_st(mine + i * TG + tg, 1 - rank, send[i]);
+            ctx.cluster_sync();
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int k = tg + TG * (lo + i);
+                const cplx r = mine[i * TG + tg];  // R+ (CTA 0) or P- (CTA 1)
+                // CTA 0: X_0 = P+ + R+, X_2 = P+ - R+;  CTA 1: X_1 = P- + R-, X_3 = P- - R-
+                const cplx x_lo = rank ? cadd(r, keep[i]) : cadd(keep[i], r);
+                const cplx x_hi = rank ? csub(r, keep[i]) : csub(keep[i], r);
+                // (bit operations, which the compiler recomputes instead of keeping sixteen
+                // loop-invariant positions in spilled registers)
+                st_stream(o + ((k + Q * rank + n / 2) & (n - 1)), cscale(x_lo, scale));
+                st_stream(o + ((k + Q * (rank + 2) + n / 2) & (n - 1)), cscale(x_hi, scale));
+            }
+            ctx.group_sync(1 + grp, TG);  // the group's exchange buffer is reused by its next line
         }
     }
 };

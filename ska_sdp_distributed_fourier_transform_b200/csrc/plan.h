@@ -28,6 +28,7 @@ struct swiftly_b200 {
     // launch ran (kernel, lines per CTA or F or chunks per tensor load, output path or
     // line-fastest flag or staging capacity, grid), see swiftly_b200_debug_last_launch
     mutable int last_launch[4];
+    mutable int last_cluster;  // CTAs per cluster of that launch (swiftly_b200_debug_last_cluster)
 };
 
 namespace swiftly {
@@ -54,7 +55,8 @@ enum {
     // staging buffer in samples
     LAUNCH_K2_TMA = 8,         // ExtractColumnsTmaKernel<yN, false>
     LAUNCH_K2_TMA_SPLIT = 9,   // ExtractColumnsTmaKernel<yN / 2, true>
-    LAUNCH_K2_TMA4 = 10,       // ExtractColumnsTma4Kernel<yN / 4>
+    LAUNCH_K2_TMA4 = 10,       // ExtractColumnsTma4Kernel<yN / 4>, or its pairs on two-CTA
+                               // clusters, ExtractColumnsClusterKernel<yN / 4> (same grid)
     LAUNCH_K2_DIF = 11,        // ExtractColumnsTmaDifKernel<yN / 4, BOTH>
     LAUNCH_K2_PARK_DIF = 12,   // ExtractColumnsParkKernel<yN / 4, 0>: facets of at most yN / 2
     LAUNCH_K2_PARK_DIF2 = 13,  // ExtractColumnsParkKernel<yN / 4, 1>: longer facets
@@ -64,11 +66,13 @@ enum {
 };
 
 // records the form of a launch for swiftly_b200_debug_last_launch (one host-side store)
-inline void note_launch(const swiftly_b200* h, int kernel, int lines, int out_path, int grid) {
+inline void note_launch(const swiftly_b200* h, int kernel, int lines, int out_path, int grid,
+                        int cluster = 1) {
     h->last_launch[0] = kernel;
     h->last_launch[1] = lines;
     h->last_launch[2] = out_path;
     h->last_launch[3] = grid;
+    h->last_cluster = cluster;
 }
 
 // SMs of the H100 SXM: grid size of the persistent kernels and cap of the grid-stride ones
