@@ -113,6 +113,15 @@ int swiftly_b200_add_to_facet(const swiftly_b200* plan, const swiftly_b200_lines
 int swiftly_b200_finish_facet(const swiftly_b200* plan, const swiftly_b200_lines* in,
                               const swiftly_b200_lines* out, int64_t facet_off,
                               const double* mask, void* stream);
+/* finish_facet of a real image: the real part only, as float64 samples,
+ *   out[k] = (Re(fft_c(in))[(yN/2 - fs//2 + k + facet_off) mod yN] * Fb[k]) * mask[k],
+ * in that product order, i.e. bitwise Re(swiftly_b200_finish_facet(mask = NULL)) * mask.
+ * in: n_lines x yN_size complex128; out: n_lines x facet_size DOUBLES (overwritten) whose
+ * line_stride and elem_stride count doubles, not complex elements.  mask: facet_size device
+ * doubles or NULL.  Device arrays only (SWIFTLY_B200_EINVAL otherwise). */
+int swiftly_b200_finish_facet_real(const swiftly_b200* plan, const swiftly_b200_lines* in,
+                                   const swiftly_b200_lines* out, int64_t facet_off,
+                                   const double* mask, void* stream);
 
 /* ---- fused forward path (device memory only) ---------------------------------------- */
 /* The reference's `extract_column` task (api_helper.py:200-210) in one kernel:
@@ -223,6 +232,19 @@ int swiftly_b200_mirror_subgrid(const swiftly_b200* plan, const swiftly_b200_lin
                                 const double* mask0, const double* mask1,
                                 const double* mirror_mask0, const double* mirror_mask1,
                                 void* stream);
+/* The adjoint of swiftly_b200_mirror_subgrid (unmasked), for the backward transform of a real
+ * image: the subgrids sg at (off0, off1) and mirror at (-off0, -off1), both sz x sz, merged into
+ * ONE subgrid of size S = 2h + 1, h = sz // 2, at (off0, off1) whose backward transform has the
+ * same real part as the sum of theirs:
+ *   out[r, c] = [r, c < sz] sg[r, c] + [2h - r, 2h - c < sz] conj(mirror[2h - r, 2h - c])
+ * for r, c < S.  Where both terms exist: one complex add; where one exists: that term
+ * unchanged; where neither does (even sz: the last row and column): 0.  out: S x S
+ * (overwritten).  Any line and element strides; device arrays only.  Reads and writes
+ * 16 * (2 sz^2 + S^2) bytes.  SWIFTLY_B200_EINVAL when sg and mirror are not both sz x sz, out
+ * is not S x S, or an array is on the host. */
+int swiftly_b200_merge_mirror_subgrid(const swiftly_b200* plan, const swiftly_b200_lines* sg,
+                                      const swiftly_b200_lines* mirror,
+                                      const swiftly_b200_lines* out, void* stream);
 /* ---- fused backward path (device memory only) --------------------------------------- */
 /* One subgrid into the column accumulators of n_facets (<= 64) facets in ONE launch: per
  * facet `extract_from_subgrid(block, facet_off1, axis=1)` followed by `accumulate_column` =

@@ -88,6 +88,7 @@ SYMBOLS = {
     "swiftly_b200_extract_from_subgrid": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_add_to_facet": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_finish_facet": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "swiftly_b200_finish_facet_real": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "swiftly_b200_extract_column": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_sum_finish_axis": (ctypes.c_int, [_PLAN, ctypes.POINTER(Source), ctypes.c_int, _LINES_P, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "swiftly_b200_sum_finish_axis_grouped": (ctypes.c_int, [_PLAN, ctypes.POINTER(Source), ctypes.POINTER(ctypes.c_int32), ctypes.c_int, _LINES_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
@@ -98,6 +99,7 @@ SYMBOLS = {
     "swiftly_b200_extract_columns": (ctypes.c_int, [_PLAN, ctypes.c_int, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.POINTER(ctypes.c_int64), ctypes.c_void_p]),
     "swiftly_b200_extract_columns_windowed": (ctypes.c_int, [_PLAN, ctypes.c_int, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.POINTER(ctypes.c_int64), ctypes.c_void_p]),
     "swiftly_b200_mirror_subgrid": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, _LINES_P, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "swiftly_b200_merge_mirror_subgrid": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, _LINES_P, ctypes.c_void_p]),
     "swiftly_b200_subgrid_to_facets": (ctypes.c_int, [_PLAN, ctypes.c_int, _LINES_P, _LINES_P, ctypes.POINTER(ctypes.c_int64), ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_fold_column": (ctypes.c_int, [_PLAN, ctypes.c_int, _LINES_P, _LINES_P, ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_void_p), ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_sum_finish_axis_supported": (ctypes.c_int, [_PLAN]),

@@ -886,11 +886,18 @@ class SwiftlyBackward:
         (:func:`device_tier_bytes`), the facet accumulators live in pinned host memory and
         the device holds only the ``m``-row window the current column adds into (the host
         tier); ``finish()`` then returns the facets in pinned host memory, the same bits
+    :param real_image: the image is real-valued: ``finish()`` returns the real part of the
+        facets as float64 (``finish_facet_real``), and :meth:`add_subgrid_tasks` merges each
+        Hermitian pair of subgrids at ``(off0, off1)`` / ``(-off0, -off1)`` into one subgrid
+        (``merge_mirror_subgrid``) before the subgrid side, which then runs once per pair.
+        Needs the fused kernels (``NotImplementedError`` otherwise).
+        :meth:`add_new_subgrid_task` is unchanged.  The sharded backward transform
+        (``SwiftlyBackwardSharded``) has no real-image mode
     """
 
     # pylint: disable=too-many-arguments,too-many-instance-attributes
     def __init__(self, swiftly_config, facets_config_list, lru_backward=1, queue_size=20,
-                 client=None, device_budget=None):
+                 client=None, device_budget=None, real_image=False):
         self.config = swiftly_config
         self.core = swiftly_config.core
         self.device = _device_of(self.core)
@@ -914,8 +921,14 @@ class SwiftlyBackward:
             rows.setdefault(cfg.off0, []).append(idx)
         self._rows = list(rows.items())
         self._row_members = dict(self._rows)
-        self._strips = None
+        # K4T strip buffers of the last two subgrid widths: real-image columns that hold
+        # self-mirrored subgrids alternate the merged width S and the subgrid width
+        self._strips = collections.OrderedDict()
         self._masks1 = None
+        self.real_image = bool(real_image)
+        if self.real_image and not self._fused:
+            raise NotImplementedError(
+                "real_image=True needs the fused backward kernels, which this core lacks")
         self.host_tier = self._fused and bool(self.facets_config_list) and device_tier_bytes(
             "backward", self.core.yN_size, self.core.xM_yN_size,
             [cfg.size for cfg in self.facets_config_list], self.lru.size,
@@ -1009,8 +1022,14 @@ class SwiftlyBackward:
             for r0, cnt in fresh:
                 cp.zero(acc[r0:r0 + cnt])
             cp.compute_waits(cp.record())
-            facet = finish_facet(core, acc, cfg)
-            out = host.reshape(-1)[:cfg.size * cfg.size].view(cfg.size, cfg.size)
+            if self.real_image:
+                # float64 facet in the first half of the accumulator's bytes: half the D2H
+                facet = self._finish_real(acc, cfg)
+                out = host.reshape(-1).view(torch.float64)[:cfg.size * cfg.size]
+            else:
+                facet = finish_facet(core, acc, cfg)
+                out = host.reshape(-1)[:cfg.size * cfg.size]
+            out = out.view(cfg.size, cfg.size)
             cp.after_compute()
             cp.copy(out, cp.use(facet), True)
             tasks.append(DeviceTask(out))
@@ -1019,8 +1038,10 @@ class SwiftlyBackward:
 
     def add_new_subgrid_task(self, subgrid_config, new_subgrid_task):
         """Fold one subgrid into the facet accumulators."""
-        off0, off1 = subgrid_config.off0, subgrid_config.off1
         subgrid = _to_device(_resolve(new_subgrid_task), self.device)
+        return self._add_subgrid(subgrid, subgrid_config.off0, subgrid_config.off1)
+
+    def _add_subgrid(self, subgrid, off0, off1):
         if self._split:
             done = self._add_subgrid_split(subgrid, off0, off1)
         elif self._fused:
@@ -1032,6 +1053,36 @@ class SwiftlyBackward:
             done = self.update_off0_NAF_MNAFs(off0, off1, pieces)
         self.task_queue.process(done)
         return done
+
+    def add_subgrid_tasks(self, subgrid_configs, subgrid_tasks):
+        """Fold every subgrid of ``subgrid_configs`` (data in ``subgrid_tasks``, the same length;
+        arrays, tensors or lazy handles, resolved when used) into the facet accumulators.
+        Returns the :func:`mirror_pairs` plan it followed.
+
+        Default: :meth:`add_new_subgrid_task` in list order, plan ``[(i, None), ...]``.  With
+        ``real_image``, each pair ``(i, j)`` is merged (``merge_mirror_subgrid``) into one subgrid
+        of size ``S = 2 * (size // 2) + 1`` at config ``i``'s offsets, which then runs the subgrid
+        side once; the facets' real part is the same.  Unpaired and self-mirrored configs are
+        added as they are.
+        """
+        configs = list(subgrid_configs)
+        datas = list(subgrid_tasks)
+        if len(configs) != len(datas):
+            raise ValueError(f"{len(configs)} subgrid configs but {len(datas)} subgrids")
+        if not self.real_image:
+            for sg, data in zip(configs, datas):
+                self.add_new_subgrid_task(sg, data)
+            return [(i, None) for i in range(len(configs))]
+        plan = mirror_pairs(configs, self.config.image_size, self.config.internal_subgrid_size)
+        for i, j in plan:
+            if j is None:
+                self.add_new_subgrid_task(configs[i], datas[i])
+                continue
+            sg, mirror = (_to_device(_resolve(datas[k]), self.device) for k in (i, j))
+            merged = self.core.merge_mirror_subgrid(sg, mirror)
+            del sg, mirror
+            self._add_subgrid(merged, configs[i].off0, configs[i].off1)
+        return plan
 
     def _column_for(self, off0):
         """Column accumulators of subgrid column ``off0`` (LRU).  When a column has to make
@@ -1060,10 +1111,15 @@ class SwiftlyBackward:
     def _add_subgrid_split(self, subgrid, off0, off1):
         # K4T: the subgrid along axis 0 into one (m, xA) strip per distinct facet off0, kept
         # C-ordered so that the axis-0 lines (columns) are adjacent in memory
-        shape = (len(self._rows), self.core.xM_yN_size, subgrid.shape[1])
-        if self._strips is None or tuple(self._strips.shape) != shape:
-            self._strips = torch.empty(shape, dtype=torch.complex128, device=self.device)
-        strips = self._strips
+        width = subgrid.shape[1]
+        strips = self._strips.get(width)
+        if strips is None:
+            strips = torch.empty((len(self._rows), self.core.xM_yN_size, width),
+                                 dtype=torch.complex128, device=self.device)
+            if len(self._strips) >= 2:
+                self._strips.popitem(last=False)
+            self._strips[width] = strips
+        self._strips.move_to_end(width)
         self.core.split_subgrid_axis(
             [subgrid], 0, [off0], [[(strips[r], row) for r, (row, _) in enumerate(self._rows)]],
             "store")
@@ -1163,9 +1219,19 @@ class SwiftlyBackward:
             # 64 GiB of finished facets never coexist
             acc = self.MNAF_BMNAFs_persist[j]
             self.MNAF_BMNAFs_persist[j] = None
-            facet = finish_facet(self.core, acc, cfg)
+            if self.real_image:
+                facet = self._finish_real(acc, cfg)
+            else:
+                facet = finish_facet(self.core, acc, cfg)
             del acc
             tasks.append(DeviceTask(facet))
         self.task_queue.process(tasks)
         self.task_queue.wait_all_done()
         return tasks
+
+    def _finish_real(self, acc, cfg):
+        """The real facet (float64) of a facet accumulator, masked inside the kernel."""
+        if acc is None:
+            return numpy.zeros((cfg.size, cfg.size))
+        return self.core.finish_facet_real(acc, cfg.off0, cfg.size, axis=0,
+                                           mask=_device_mask(cfg.mask0, self.device))

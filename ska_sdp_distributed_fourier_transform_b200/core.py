@@ -698,6 +698,75 @@ class SwiftlyCoreB200:
         _lib.check(self._lib, rc)
         return outs[0], outs[1]
 
+    def merge_mirror_subgrid(self, sg, mirror, out=None):
+        """One subgrid in place of a Hermitian pair (real image), the adjoint of
+        :meth:`mirror_subgrid`.
+
+        ``sg`` / ``mirror``: the ``(sz, sz)`` subgrids at ``(off0, off1)`` and ``(-off0, -off1)``.
+        Returns the ``(S, S)`` subgrid at ``(off0, off1)``, ``S = 2 * (sz // 2) + 1``,
+        ``out[r, c] = sg[r, c] + conj(mirror[2h - r, 2h - c])`` (each term where its indices are
+        below ``sz``, 0 where neither is), whose backward transform has the real part of the sum
+        of the pair's.  ``out`` may be given (any strides); complex128 device tensors only.
+        """
+        for t in (sg, mirror):
+            self._check_tensor(t)
+            if t.dtype != torch.complex128 or t.dim() != 2:
+                raise ValueError("merge_mirror_subgrid needs 2-D complex128 device tensors")
+        sz = int(sg.shape[0])
+        if tuple(sg.shape) != (sz, sz) or tuple(mirror.shape) != (sz, sz):
+            raise ValueError(f"sg and mirror must both be square of one size, got "
+                             f"{tuple(sg.shape)} and {tuple(mirror.shape)}")
+        S = 2 * (sz // 2) + 1
+        if out is None:
+            out = torch.empty((S, S), dtype=torch.complex128, device=sg.device)
+        self._check_tensor(out)
+        if out.dtype != torch.complex128 or tuple(out.shape) != (S, S):
+            raise ValueError(f"Output array has shape {tuple(out.shape)}, expected {(S, S)}!")
+        dsg, dmir, dout = (self._describe(t, 1) for t in (sg, mirror, out))
+        rc = self._lib.swiftly_b200_merge_mirror_subgrid(
+            self._plan, ctypes.byref(dsg), ctypes.byref(dmir), ctypes.byref(dout),
+            self._stream(sg))
+        _lib.check(self._lib, rc)
+        return out
+
+    def finish_facet_real(self, MiNjSi_sum, facet_off, facet_size, axis, out=None, mask=None):
+        """:meth:`finish_facet` of a real image: the real part only, float64.
+
+        ``out[k] = (Re(finish_facet(...))[k]) * mask[k]`` bitwise (the window product first, the
+        mask after, as ``finish_facet`` followed by a row mask).  ``MiNjSi_sum``: 2-D complex128
+        device tensor; ``out``: float64 device tensor of the finished shape (any strides) or None;
+        ``mask``: None or ``facet_size`` samples.
+        """
+        acc = MiNjSi_sum
+        self._check_tensor(acc)
+        if acc.dtype != torch.complex128 or acc.dim() != 2:
+            raise ValueError("finish_facet_real needs a 2-D complex128 device tensor")
+        if axis not in (0, 1):
+            raise ValueError(f"Invalid axis {axis} for shape {tuple(acc.shape)}!")
+        shape = list(acc.shape)
+        shape[axis] = int(facet_size)
+        shape = tuple(shape)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float64, device=acc.device)
+        self._check_tensor(out)
+        if out.dtype != torch.float64 or tuple(out.shape) != shape:
+            raise ValueError(f"Output array has shape {tuple(out.shape)} and dtype {out.dtype}, "
+                             f"expected {shape} float64!")
+        keep = []
+        mptr = ctypes.c_void_p(0)
+        if mask is not None:
+            mptr = self._mask_ptr(mask, out, keep)
+            if keep[0].numel() != shape[axis]:
+                raise ValueError("mask must have the facet size")
+        other = 1 - axis
+        dout = _lib.Lines(out.data_ptr(), shape[other], shape[axis], out.stride(other),
+                          out.stride(axis), _lib.DEVICE)
+        rc = self._lib.swiftly_b200_finish_facet_real(
+            self._plan, ctypes.byref(self._describe(acc, axis)), ctypes.byref(dout),
+            int(facet_off), mptr, self._stream(acc))
+        _lib.check(self._lib, rc)
+        return out
+
     def release_scratch(self):
         """Give the plan's scratch buffers (2 GiB after stage 1 at N = 65536) back to the device."""
         self._lib.swiftly_b200_release_scratch(self._plan)

@@ -212,8 +212,8 @@ extern "C" void swiftly_b200_debug_sg_variant(swiftly_b200* h, int variant) {
 // extract_columns kernels: 8 ExtractColumnsTmaKernel<yN, false>, 9 its 2 x yN/2 split,
 // 10 ExtractColumnsTma4Kernel, 11 ExtractColumnsTmaDifKernel, 12 / 13 / 14
 // ExtractColumnsParkKernel MODE 0 / 1 / 2, 15 ExtractColumnsParkSkewKernel; 16
-// MirrorSubgridKernel, with 0 in out[1] and out[2]); out[1]: lines per
-// CTA (1 .. 4), F (5, 6: 2 for SplitLineKernel), 0 (7), or for 8 .. 15 the 128-byte chunks per
+// MirrorSubgridKernel and 17 MergeMirrorSubgridKernel, with 0 in out[1] and out[2]); out[1]:
+// lines per CTA (1 .. 4), F (5, 6: 2 for SplitLineKernel), 0 (7), or for 8 .. 15 the 128-byte chunks per
 // tensor load when the rows are staged swizzled and 0 when they are staged by linear bulk
 // copies; out[2]: output path of the fused kernels (0 direct stores, 1 TMA with one tensor map,
 // 2 TMA with one tensor map per group), the line-fastest flag of 4 and 7, 0 for 5 and 6, the
@@ -608,4 +608,39 @@ extern "C" int swiftly_b200_finish_facet(const swiftly_b200* h, const swiftly_b2
     op.mask = sm.dev;
     SW_TRY(run_finish_facet(h, op, lines_adjacent(g), s));
     return stage_out(sout, s);
+}
+
+extern "C" int swiftly_b200_finish_facet_real(const swiftly_b200* h,
+                                              const swiftly_b200_lines* in,
+                                              const swiftly_b200_lines* out, int64_t facet_off,
+                                              const double* mask, void* stream) {
+    if (!h) return einval("finish_facet_real: NULL plan");
+    SW_TRY(check_lines(in, out, h->yN, -1, "finish_facet_real"));
+    if (in->location != SWIFTLY_B200_DEVICE || out->location != SWIFTLY_B200_DEVICE)
+        return einval("finish_facet_real: device arrays only");
+    const int64_t yN = h->yN, fs = out->size;
+    if (fs > yN - 1) return einval("finish_facet_real: facet size must be at most yN_size - 1");
+    if (in->n_lines == 0) return SWIFTLY_B200_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    SW_DEVICE_GUARD(h);
+    FinishFacetRealOp op;
+    op.g.in = (const cplx*)in->data;
+    op.g.out = nullptr;
+    op.g.in_ls = in->line_stride;
+    op.g.in_es = in->elem_stride;
+    // (strides in doubles: only their adjacency enters the choice of the kernel form)
+    op.g.out_ls = out->line_stride;
+    op.g.out_es = out->elem_stride;
+    op.g.n_lines = in->n_lines;
+    op.fb = h->d_Fb + ((yN - 1) / 2 - fs / 2);
+    op.n = (int)yN;
+    op.fs = (int)fs;
+    op.start = (int)pmod(yN / 2 - fs / 2 + facet_off, yN);
+    op.mask = nullptr;
+    op.rout = (double*)out->data;
+    op.rout_ls = out->line_stride;
+    op.rout_es = out->elem_stride;
+    op.rmask = mask;
+    SW_TRY(run_finish_facet(h, op, lines_adjacent(op.g), s));
+    return SWIFTLY_B200_OK;
 }

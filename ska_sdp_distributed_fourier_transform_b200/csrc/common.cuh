@@ -83,6 +83,13 @@ SW_HD void st_stream(cplx* p, cplx v) {
     *p = v;
 #endif
 }
+SW_HD void st_stream_d(double* p, double v) {
+#if defined(__CUDA_ARCH__)
+    __stcs(p, v);
+#else
+    *p = v;
+#endif
+}
 
 // two adjacent samples (32 bytes, 32-byte aligned): one 32-byte sector per thread, written by
 // two streaming 16-byte stores (sm_90 has no 256-bit global store)

@@ -1,32 +1,10 @@
 // SwiFTly -- size dispatch of finish_facet (one translation unit per primitive keeps
 // the heavy FP64 template instantiations compiling in parallel).
-#include "dispatch.cuh"
+#include "dispatch_finish_facet.cuh"
 
 namespace swiftly {
 
-int run_finish_facet(const swiftly_b200* h, const FinishFacetOp& op, bool lf, cudaStream_t s) {
-    const int n = op.n;
-    if (h->force_split && n >= 2 * MIN_FFT && n <= MAX_DIRECT_FFT) {
-        switch (n) {
-#if defined(SWIFTLY_EMU)
-            case 128: return launch_split<64, -1, FinishFacetOp>(h, op, s);
-            case 512: return launch_split<256, -1, FinishFacetOp>(h, op, s);
-#endif
-            default: break;
-        }
-    }
-    switch (n) {
-        SW_DIRECT_CASES(-1, FinishFacetOp)
-        case 16384: return launch_split<8192, -1, FinishFacetOp>(h, op, s);
-        default: break;
-    }
-    {
-        int M = 0, F = 0;
-        if (split_f_plan(n, &M, &F)) {
-            SW_SPLIT_F_CASES(-1, FinishFacetOp, M, F)
-        }
-    }
-    return unsupported(n);
-}
+template int run_finish_facet<FinishFacetOp>(const swiftly_b200*, const FinishFacetOp&, bool,
+                                             cudaStream_t);
 
 }  // namespace swiftly

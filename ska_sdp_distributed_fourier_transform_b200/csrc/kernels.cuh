@@ -302,6 +302,25 @@ struct FinishFacetOp {
     }
 };
 
+// finish_facet of a real image: out[k] = (Re(fft_c(sum))[...] * Fb_c[k]) * mask[k], written as
+// doubles.  The product order is that of finish_facet followed by the driver's row mask
+// (api_helper.py finish_facet), so the samples are bitwise Re of the complex facet's.  g.out and
+// mask are unused; the output strides are counted in doubles.
+struct FinishFacetRealOp : FinishFacetOp {
+    double* rout;
+    int64_t rout_ls, rout_es;
+    const double* rmask;  // optional facet mask along the axis, or null
+    SW_HD void store(int64_t line, int p, cplx v) const {
+        int pc = wrap_add(p, n / 2, n);
+        int k = wrap_sub(pc, start, n);
+        if (k < fs) {
+            double x = v.x * ldg_d(fb + k);
+            if (rmask) x *= ldg_d(rmask + k);
+            st_stream_d(rout + line * rout_ls + (int64_t)k * rout_es, x);
+        }
+    }
+};
+
 // add_to_subgrid (core.py:255-285):
 //   out[(xM/2 - m/2 + u + sf) mod xM] += Fn[u] * fft_c(contrib)[(u + sf) mod m]
 struct AddToSubgridOp {

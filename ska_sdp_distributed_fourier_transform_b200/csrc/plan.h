@@ -62,7 +62,8 @@ enum {
     LAUNCH_K2_PARK_DIF2 = 13,  // ExtractColumnsParkKernel<yN / 4, 1>: longer facets
     LAUNCH_K2_PARK_DIT = 14,   // ExtractColumnsParkKernel<yN / 4, 2>
     LAUNCH_K2_PARK_SKEW = 15,  // ExtractColumnsParkSkewKernel<yN / 4>
-    LAUNCH_MIRROR = 16         // MirrorSubgridKernel (dispatch_mirror_subgrid.cu): 0, 0
+    LAUNCH_MIRROR = 16,        // MirrorSubgridKernel (dispatch_mirror_subgrid.cu): 0, 0
+    LAUNCH_MERGE_MIRROR = 17   // MergeMirrorSubgridKernel (dispatch_merge_mirror_subgrid.cu): 0, 0
 };
 
 // records the form of a launch for swiftly_b200_debug_last_launch (one host-side store)
@@ -86,7 +87,9 @@ inline bool is_pow2(int64_t n) { return n > 0 && (n & (n - 1)) == 0; }
 // dispatchers, one translation unit each (compile time!): launch `op` over all
 // its lines with an n-point transform.  dir = -1 forward, +1 inverse.
 int run_prepare_facet(const swiftly_b200* h, const PrepareFacetOp& op, bool line_fastest, cudaStream_t s);
-int run_finish_facet(const swiftly_b200* h, const FinishFacetOp& op, bool line_fastest, cudaStream_t s);
+// FinishFacetOp or FinishFacetRealOp (dispatch_finish_facet.cuh)
+template <class Op>
+int run_finish_facet(const swiftly_b200* h, const Op& op, bool line_fastest, cudaStream_t s);
 int run_add_to_subgrid(const swiftly_b200* h, const AddToSubgridOp& op, bool line_fastest, cudaStream_t s);
 int run_extract_from_subgrid(const swiftly_b200* h, const ExtractFromSubgridOp& op, bool line_fastest, cudaStream_t s);
 int run_finish_subgrid(const swiftly_b200* h, const FinishSubgridOp& op, bool line_fastest, cudaStream_t s);
