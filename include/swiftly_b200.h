@@ -122,6 +122,14 @@ int swiftly_b200_finish_facet(const swiftly_b200* plan, const swiftly_b200_lines
 int swiftly_b200_finish_facet_real(const swiftly_b200* plan, const swiftly_b200_lines* in,
                                    const swiftly_b200_lines* out, int64_t facet_off,
                                    const double* mask, void* stream);
+/* swiftly_b200_finish_facet_real of a line kept as half rows (see "Half rows" below): in has
+ * yN_size/2 + 1 samples per line, stored sample q being natural FFT index q.  The transform input
+ * is the Hermitian part of the full line, 0.5 in[q] (0 < q < yN/2), 0.5 conj(in[yN - q])
+ * (q > yN/2), (Re in[q], 0) (q = 0, yN/2): bitwise swiftly_b200_finish_facet_real of the full
+ * line built that way.  Same contract otherwise; SWIFTLY_B200_EINVAL for an odd yN_size. */
+int swiftly_b200_finish_facet_real_half(const swiftly_b200* plan, const swiftly_b200_lines* in,
+                                        const swiftly_b200_lines* out, int64_t facet_off,
+                                        const double* mask, void* stream);
 
 /* ---- fused forward path (device memory only) ---------------------------------------- */
 /* The reference's `extract_column` task (api_helper.py:200-210) in one kernel:
@@ -200,6 +208,15 @@ int swiftly_b200_peer_wait(const swiftly_b200* plan, const void* my_flags, int n
  * bf_f[f] (every facet_accs[f]) has yN_size lines, or every one has xM_yN_size lines; any other
  * line count is rejected.  A ring runs the same kernel form as the whole array with the same
  * facet size and row stride. */
+/* Half rows.  For a real image every column of BF_F (and the part of a facet accumulator that
+ * finish_facet_real reads) is conjugate-symmetric in the centred row index: rows yN/2 + d and
+ * yN/2 - d are conjugates.  A caller may then pass yN_size/2 + 1 rows (yN_size even): stored row
+ * d, 0 <= d <= yN/2, holds centred row (yN/2 + d) mod yN.  Centred row r is stored row
+ * i = (r - yN/2) mod yN when that is <= yN/2, else yN - i, conjugated.  extract_columns[_windowed]
+ * reads a conjugated row with every imaginary part negated (bitwise the call on the full
+ * Hermitian rows); fold_column adds conj(w v) into a conjugated row, w v elsewhere, in at most two
+ * passes in stream order: a window across centred offset 0 or yN/2 holds rows r and -r, and the
+ * unconjugated one is added first.  One call takes half rows for every facet or for none. */
 /* swiftly_b200_extract_column for n_facets (<= 64) facets in ONE launch: bf_f[f] / out[f]
  * as in swiftly_b200_extract_column (contiguous rows, or row rings), facet_off1[f] per facet. */
 int swiftly_b200_extract_columns(const swiftly_b200* plan, int n_facets,
@@ -217,6 +234,15 @@ int swiftly_b200_extract_columns_windowed(const swiftly_b200* plan, int n_facets
                                           const swiftly_b200_lines* bf_f,
                                           const swiftly_b200_lines* out, int64_t subgrid_off0,
                                           const int64_t* facet_off1, void* stream);
+/* swiftly_b200_prepare_facet_windowed of a REAL facet, keeping only its half rows (see "Half
+ * rows" below): in: n_lines x facet_size DOUBLES (line_stride and elem_stride count doubles);
+ * out: n_lines x (yN_size/2 + 1) complex128, line l sample d = the windowed prepared facet's
+ * line l at centred index (yN/2 + d) mod yN.  Bitwise equal to those samples of
+ * swiftly_b200_prepare_facet_windowed applied to the facet promoted to complex.  Device arrays
+ * only; SWIFTLY_B200_EINVAL for an odd yN_size. */
+int swiftly_b200_prepare_facet_real_half(const swiftly_b200* plan, const swiftly_b200_lines* in,
+                                         const swiftly_b200_lines* out, int64_t facet_off,
+                                         void* stream);
 /* The two finished subgrids of a Hermitian pair (real image: G(-u, -v) = conj(G(u, v))) from
  * ONE unmasked source, finish_subgrid (core.py:287-325) with api_helper.py:107-111's masks:
  *   out[r, c]    = mask0[r] * mask1[c] * src[r, c]

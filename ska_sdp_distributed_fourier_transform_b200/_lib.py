@@ -89,6 +89,8 @@ SYMBOLS = {
     "swiftly_b200_add_to_facet": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_finish_facet": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "swiftly_b200_finish_facet_real": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "swiftly_b200_finish_facet_real_half": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "swiftly_b200_prepare_facet_real_half": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_extract_column": (ctypes.c_int, [_PLAN, _LINES_P, _LINES_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p]),
     "swiftly_b200_sum_finish_axis": (ctypes.c_int, [_PLAN, ctypes.POINTER(Source), ctypes.c_int, _LINES_P, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     "swiftly_b200_sum_finish_axis_grouped": (ctypes.c_int, [_PLAN, ctypes.POINTER(Source), ctypes.POINTER(ctypes.c_int32), ctypes.c_int, _LINES_P, ctypes.c_int64, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),

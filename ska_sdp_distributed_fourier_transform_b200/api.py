@@ -305,7 +305,7 @@ def _to_device(data, device, dtype=None):
     return torch.from_numpy(numpy.ascontiguousarray(arr)).to(device, non_blocking=True)
 
 
-def _upload_iter(datas, device):
+def _upload_iter(datas, device, dtype=None):
     """Yield device tensors for ``datas`` in order.
 
     Host sources are uploaded on a side stream one item ahead of the consumer, so that the
@@ -319,11 +319,11 @@ def _upload_iter(datas, device):
     def upload(data):
         data = _resolve(data)
         if isinstance(data, torch.Tensor) and data.device == device:
-            return _to_device(data, device), None
+            return _to_device(data, device, dtype), None
         if not use_side:
-            return _to_device(data, device), None
+            return _to_device(data, device, dtype), None
         with torch.cuda.stream(side):
-            t = _to_device(data, device)
+            t = _to_device(data, device, dtype)
             ev = torch.cuda.Event()
             ev.record(side)
         return t, ev
@@ -340,7 +340,8 @@ def _upload_iter(datas, device):
 
 
 # ---------------------------------------------------------------------- host tier
-def device_tier_bytes(direction, yN, m, facet_sizes, lru, n_rows=0, subgrid_size=0):
+def device_tier_bytes(direction, yN, m, facet_sizes, lru, n_rows=0, subgrid_size=0,
+                      half_rows=False):
     """Bytes of device memory the device tier of a one-GPU transform holds at its peak.
 
     ``"forward"``: every prepared facet ``BF_F`` (``yN x size``), ``lru`` subgrid columns of
@@ -348,10 +349,11 @@ def device_tier_bytes(direction, yN, m, facet_sizes, lru, n_rows=0, subgrid_size
     stage-1 scratch (one ``yN x size`` facet).  ``"backward"``: every facet accumulator
     (``yN x size``) and ``lru`` columns of accumulators (``m x yN`` per facet).  When this exceeds
     the device budget, :class:`SwiftlyForward` / :class:`SwiftlyBackward` keep those facet arrays
-    in pinned host memory instead (the host tier).
+    in pinned host memory instead (the host tier).  ``half_rows``: the facet arrays have
+    ``yN // 2 + 1`` rows (real images, ``half_rows=True`` of the transforms).
     """
     sizes = list(facet_sizes)
-    facets = 16 * yN * sum(sizes)
+    facets = 16 * (yN // 2 + 1 if half_rows else yN) * sum(sizes)
     columns = 16 * max(1, int(lru)) * len(sizes) * m * yN
     if direction == "backward":
         return facets + columns
@@ -544,6 +546,20 @@ def _real_facet(idx, data):
     return data
 
 
+def _half_rows_mode(half_rows, real_image):
+    if half_rows and not real_image:
+        raise ValueError("half_rows=True is valid only together with real_image=True")
+    return bool(half_rows)
+
+
+def _half_rows_budget(need, budget):
+    """The half-row mode runs in the device tier only."""
+    if need > budget:
+        raise NotImplementedError(
+            f"half_rows=True runs in the device tier only: it needs an estimated {need} bytes "
+            f"of device memory, the budget is {budget} bytes")
+
+
 def mirror_pairs(subgrid_configs, N, xM):
     """How the real-image forward transform covers ``subgrid_configs``: a list of
     ``(i, j)`` in the order of the sources ``i``, where ``j`` is the index of the config whose
@@ -603,11 +619,18 @@ class SwiftlyForward:
         :meth:`iter_subgrid_tasks` computes one subgrid of each pair at ``(off0, off1)`` /
         ``(-off0, -off1)`` and mirrors the other (:func:`mirror_pairs`).  Needs the fused
         kernels (``NotImplementedError`` otherwise).  :meth:`get_subgrid_task` is unchanged
+    :param half_rows: with ``real_image`` only (``ValueError`` otherwise): every prepared facet
+        is kept as its ``yN // 2 + 1`` half rows (``prepare_facet_real_half``; the other rows are
+        their conjugates), half the device memory of the facet arrays.  The facets are uploaded
+        as float64.  Device tier only: ``NotImplementedError`` when :func:`device_tier_bytes`
+        with ``half_rows=True`` exceeds the budget or ``bf_f_buffers`` are host tensors;
+        ``bf_f_buffers`` must have the half shape.  The subgrids differ from ``real_image`` alone
+        by rounding only
     """
 
     # pylint: disable=too-many-arguments,too-many-instance-attributes
     def __init__(self, swiftly_config, facet_tasks, lru_forward=1, queue_size=20, client=None,
-                 bf_f_buffers=None, device_budget=None, real_image=False):
+                 bf_f_buffers=None, device_budget=None, real_image=False, half_rows=False):
         self.config = swiftly_config
         self.facet_tasks = list(facet_tasks)
         self.core = swiftly_config.core
@@ -627,12 +650,24 @@ class SwiftlyForward:
         self._masks = {}
         self._fused = bool(getattr(self.core, "fused_forward_supported", lambda: False)())
         self.real_image = bool(real_image)
+        self.half_rows = _half_rows_mode(half_rows, self.real_image)
         if self.real_image:
             if not self._fused:
                 raise NotImplementedError(
                     "real_image=True needs the fused forward kernels, which this core lacks")
             self.facet_tasks = [(cfg, _real_facet(idx, data))
                                 for idx, (cfg, data) in enumerate(self.facet_tasks)]
+        if self.half_rows and bf_f_buffers is not None:
+            for (cfg, _), buf in zip(self.facet_tasks, bf_f_buffers):
+                if buf.device != self.device:
+                    raise NotImplementedError(
+                        "half_rows=True runs in the device tier only: bf_f_buffers must be "
+                        f"tensors on {self.device}")
+                shape = (self.core.half_rows, cfg.size)
+                if tuple(buf.shape) != shape or buf.dtype != torch.complex128:
+                    raise ValueError(f"half_rows=True: bf_f_buffers entry of shape "
+                                     f"{tuple(buf.shape)} and dtype {buf.dtype}, expected "
+                                     f"{shape} complex128")
         self.host_tier = self._fused and self._select_host_tier(device_budget)
         self.arena = None
         self._rings = None
@@ -650,8 +685,12 @@ class SwiftlyForward:
         core = self.core
         sizes = [cfg.size for cfg, _ in self.facet_tasks]
         need = device_tier_bytes("forward", core.yN_size, core.xM_yN_size, sizes, self.lru.size,
-                                 len(self._rows), self.config.max_subgrid_size)
-        return need > _device_budget(self.device, device_budget)
+                                 len(self._rows), self.config.max_subgrid_size,
+                                 half_rows=self.half_rows)
+        budget = _device_budget(self.device, device_budget)
+        if self.half_rows:
+            _half_rows_budget(need, budget)
+        return need > budget
 
     @property
     def copied_bytes(self):
@@ -693,10 +732,17 @@ class SwiftlyForward:
             self.facet_tasks = [(cfg, None) for cfg, _ in self.facet_tasks]
         if self.BF_Fs_persist is None:
             out = []
-            uploads = _upload_iter([data for _, data in self.facet_tasks], self.device)
+            uploads = _upload_iter([data for _, data in self.facet_tasks], self.device,
+                                   torch.float64 if self.half_rows else None)
             for idx, ((cfg, _), facet) in enumerate(zip(self.facet_tasks, uploads)):
                 buf = None if self._bf_f_buffers is None else self._bf_f_buffers[idx]
-                if self._fused:
+                if self.half_rows:
+                    # float64 with adjacent columns (a .real view of a complex facet has none),
+                    # so that K1 takes its two-pass form
+                    facet = facet.to(torch.float64).contiguous()
+                    out.append(self.core.prepare_facet_real_half(facet, cfg.off0, axis=0,
+                                                                 out=buf))
+                elif self._fused:
                     # pre-windowed along axis 1 (the K2 kernel then skips its Fb multiply)
                     out.append(self.core.prepare_facet(facet, cfg.off0, axis=0, out=buf,
                                                        window_lines=True))
@@ -893,11 +939,17 @@ class SwiftlyBackward:
         Needs the fused kernels (``NotImplementedError`` otherwise).
         :meth:`add_new_subgrid_task` is unchanged.  The sharded backward transform
         (``SwiftlyBackwardSharded``) has no real-image mode
+    :param half_rows: with ``real_image`` only (``ValueError`` otherwise): the facet accumulators
+        hold ``yN // 2 + 1`` half rows (``fold_column`` adds the conjugate of the rows it
+        mirrors, ``finish_facet_real_half`` finishes them), half their device memory.  Device
+        tier only: ``NotImplementedError`` when :func:`device_tier_bytes` with
+        ``half_rows=True`` exceeds the budget.  The facets differ from ``real_image`` alone by
+        rounding only
     """
 
     # pylint: disable=too-many-arguments,too-many-instance-attributes
     def __init__(self, swiftly_config, facets_config_list, lru_backward=1, queue_size=20,
-                 client=None, device_budget=None, real_image=False):
+                 client=None, device_budget=None, real_image=False, half_rows=False):
         self.config = swiftly_config
         self.core = swiftly_config.core
         self.device = _device_of(self.core)
@@ -926,13 +978,18 @@ class SwiftlyBackward:
         self._strips = collections.OrderedDict()
         self._masks1 = None
         self.real_image = bool(real_image)
+        self.half_rows = _half_rows_mode(half_rows, self.real_image)
         if self.real_image and not self._fused:
             raise NotImplementedError(
                 "real_image=True needs the fused backward kernels, which this core lacks")
-        self.host_tier = self._fused and bool(self.facets_config_list) and device_tier_bytes(
+        need = device_tier_bytes(
             "backward", self.core.yN_size, self.core.xM_yN_size,
             [cfg.size for cfg in self.facets_config_list], self.lru.size,
-        ) > _device_budget(self.device, device_budget)
+            half_rows=self.half_rows)
+        budget = _device_budget(self.device, device_budget)
+        if self.half_rows and self.facets_config_list:
+            _half_rows_budget(need, budget)
+        self.host_tier = self._fused and bool(self.facets_config_list) and need > budget
         self.arena = None
         self._rings = None
         self._window = None
@@ -1190,8 +1247,9 @@ class SwiftlyBackward:
             core = self.core
             for j, cfg in enumerate(self.facets_config_list):
                 if self.MNAF_BMNAFs_persist[j] is None:
+                    rows = core.half_rows if self.half_rows else core.yN_size
                     self.MNAF_BMNAFs_persist[j] = torch.zeros(
-                        (core.yN_size, cfg.size), dtype=torch.complex128, device=self.device)
+                        (rows, cfg.size), dtype=torch.complex128, device=self.device)
             if self._masks1 is None:
                 self._masks1 = [_device_mask(cfg.mask1, self.device)
                                 for cfg in self.facets_config_list]
@@ -1233,5 +1291,5 @@ class SwiftlyBackward:
         """The real facet (float64) of a facet accumulator, masked inside the kernel."""
         if acc is None:
             return numpy.zeros((cfg.size, cfg.size))
-        return self.core.finish_facet_real(acc, cfg.off0, cfg.size, axis=0,
-                                           mask=_device_mask(cfg.mask0, self.device))
+        finish = self.core.finish_facet_real_half if self.half_rows else self.core.finish_facet_real
+        return finish(acc, cfg.off0, cfg.size, axis=0, mask=_device_mask(cfg.mask0, self.device))

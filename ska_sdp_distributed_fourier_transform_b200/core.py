@@ -338,6 +338,42 @@ class SwiftlyCoreB200:
         fn = "swiftly_b200_prepare_facet_windowed" if window_lines else "swiftly_b200_prepare_facet"
         return self._run(fn, facet, self.yN_size, axis, out, facet_off)
 
+    @property
+    def half_rows(self):
+        """Rows of a half-row array of a real image: ``yN_size // 2 + 1`` (include/swiftly_b200.h,
+        "Half rows"); stored row ``d`` holds centred row ``(yN_size // 2 + d) mod yN_size``."""
+        return self.yN_size // 2 + 1
+
+    def prepare_facet_real_half(self, facet, facet_off, axis=0, out=None):
+        """``prepare_facet(facet, facet_off, axis, window_lines=True)`` of a REAL facet, keeping only
+        the half rows: along ``axis`` ``yN_size // 2 + 1`` samples, sample ``d`` being the prepared
+        facet's centred index ``(yN_size // 2 + d) mod yN_size``.  Bitwise those samples of the
+        complex call on the promoted facet; the others are their conjugates.  ``facet``: 2-D
+        float64 device tensor; ``out``: complex128 device tensor of the half shape or None.
+        """
+        if not _is_tensor(facet) or facet.dtype != torch.float64 or facet.dim() != 2:
+            raise ValueError("prepare_facet_real_half needs a 2-D float64 device tensor")
+        self._check_tensor(facet)
+        if axis not in (0, 1):
+            raise ValueError(f"Invalid axis {axis} for shape {tuple(facet.shape)}!")
+        shape = list(facet.shape)
+        shape[axis] = self.half_rows
+        shape = tuple(shape)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.complex128, device=facet.device)
+        self._check_tensor(out)
+        if out.dtype != torch.complex128 or tuple(out.shape) != shape:
+            raise ValueError(f"Output array has shape {tuple(out.shape)} and dtype {out.dtype}, "
+                             f"expected {shape} complex128!")
+        other = 1 - axis
+        din = _lib.Lines(facet.data_ptr(), facet.shape[other], facet.shape[axis],
+                         facet.stride(other), facet.stride(axis), _lib.DEVICE)
+        rc = self._lib.swiftly_b200_prepare_facet_real_half(
+            self._plan, ctypes.byref(din), ctypes.byref(self._describe(out, axis)),
+            int(facet_off), self._stream(facet))
+        _lib.check(self._lib, rc)
+        return out
+
     def extract_from_facet(self, prep_facet, subgrid_off, axis, out=None):
         """Extract the facet contribution to a subgrid (core.py:224-253)."""
         return self._run(
@@ -462,12 +498,14 @@ class SwiftlyCoreB200:
     def extract_columns(self, BF_Fs, subgrid_off0, facet_off1s, outs=None, prewindowed=False):
         """``extract_column`` for a list of facets in ONE kernel launch (<= 64 per launch).
 
-        ``prewindowed``: the ``BF_Fs`` were made with ``prepare_facet(..., window_lines=True)``.
-        Every ``BF_F`` is a whole ``(yN_size, size)`` prepared facet, or every one is an
-        ``(xM_yN_size, size)`` row ring holding row ``r`` of the column's window at line
-        ``r mod xM_yN_size`` (include/swiftly_b200.h, "Row rings").
+        ``prewindowed``: the ``BF_Fs`` were made with ``prepare_facet(..., window_lines=True)``
+        (or :meth:`prepare_facet_real_half`).  Every ``BF_F`` is a whole ``(yN_size, size)``
+        prepared facet, or every one is an ``(xM_yN_size, size)`` row ring holding row ``r`` of the
+        column's window at line ``r mod xM_yN_size`` (include/swiftly_b200.h, "Row rings"), or
+        every one holds the ``yN_size // 2 + 1`` half rows of a real image ("Half rows").
         """
         shape = (self.xM_yN_size, self.yN_size)
+        rows = (self.yN_size, self.xM_yN_size, self.half_rows)
         BF_Fs = list(BF_Fs)
         if outs is None:
             outs = [None] * len(BF_Fs)
@@ -486,6 +524,9 @@ class SwiftlyCoreB200:
                 self._check_tensor(o)
                 if b.dtype != torch.complex128 or b.dim() != 2 or b.stride(1) != 1:
                     raise ValueError("extract_columns needs row-contiguous complex128 tensors")
+                if b.shape[0] not in rows:
+                    raise ValueError(f"prepared facet has {b.shape[0]} rows, expected {rows[0]} "
+                                     f"(or a ring of {rows[1]}, or {rows[2]} half rows)!")
                 if tuple(o.shape) != shape or o.stride(1) != 1:
                     raise ValueError(f"Output array has shape {tuple(o.shape)}, expected {shape}!")
                 din[k] = self._describe(b, 1)
@@ -737,7 +778,9 @@ class SwiftlyCoreB200:
         device tensor; ``out``: float64 device tensor of the finished shape (any strides) or None;
         ``mask``: None or ``facet_size`` samples.
         """
-        acc = MiNjSi_sum
+        return self._finish_real(MiNjSi_sum, facet_off, facet_size, axis, out, mask, False)
+
+    def _finish_real(self, acc, facet_off, facet_size, axis, out, mask, half):
         self._check_tensor(acc)
         if acc.dtype != torch.complex128 or acc.dim() != 2:
             raise ValueError("finish_facet_real needs a 2-D complex128 device tensor")
@@ -761,11 +804,21 @@ class SwiftlyCoreB200:
         other = 1 - axis
         dout = _lib.Lines(out.data_ptr(), shape[other], shape[axis], out.stride(other),
                           out.stride(axis), _lib.DEVICE)
-        rc = self._lib.swiftly_b200_finish_facet_real(
-            self._plan, ctypes.byref(self._describe(acc, axis)), ctypes.byref(dout),
-            int(facet_off), mptr, self._stream(acc))
+        entry = (self._lib.swiftly_b200_finish_facet_real_half if half
+                 else self._lib.swiftly_b200_finish_facet_real)
+        rc = entry(self._plan, ctypes.byref(self._describe(acc, axis)), ctypes.byref(dout),
+                   int(facet_off), mptr, self._stream(acc))
         _lib.check(self._lib, rc)
         return out
+
+    def finish_facet_real_half(self, MiNjSi_sum, facet_off, facet_size, axis, out=None,
+                               mask=None):
+        """:meth:`finish_facet_real` of an accumulator kept as half rows: ``yN_size // 2 + 1``
+        samples along ``axis`` (include/swiftly_b200.h, "Half rows").  Bitwise
+        :meth:`finish_facet_real` of the full line whose natural-order samples are ``0.5 H[q]``,
+        ``0.5 conj(H[yN - q])`` and ``(Re H[q], 0)`` at ``q = 0, yN/2``.
+        """
+        return self._finish_real(MiNjSi_sum, facet_off, facet_size, axis, out, mask, True)
 
     def release_scratch(self):
         """Give the plan's scratch buffers (2 GiB after stage 1 at N = 65536) back to the device."""
@@ -887,19 +940,20 @@ class SwiftlyCoreB200:
         ``add_to_facet(., subgrid_off0, axis=0, out=facet_acc)`` (api_helper.py:155-179).
         ``facet_accs[f]``: ``(yN_size, facet_size)``, added to; or, for every facet, an
         ``(xM_yN_size, facet_size)`` row ring holding row ``r`` of the column's window at line
-        ``r mod xM_yN_size`` (include/swiftly_b200.h, "Row rings"); ``masks1[f]``: float64
+        ``r mod xM_yN_size`` (include/swiftly_b200.h, "Row rings"), or every one holds the
+        ``yN_size // 2 + 1`` half rows of a real image ("Half rows"); ``masks1[f]``: float64
         device tensor of the facet size or None.
         """
-        m, yN = self.xM_yN_size, self.yN_size
+        m, yN, half = self.xM_yN_size, self.yN_size, self.half_rows
 
         def chk_a(t):
             if tuple(t.shape) != (m, yN):
                 raise ValueError(f"accumulator has shape {tuple(t.shape)}, expected {(m, yN)}!")
 
         def chk_f(t):
-            if t.shape[0] not in (yN, m):
+            if t.shape[0] not in (yN, m, half):
                 raise ValueError(f"facet accumulator has {t.shape[0]} rows, expected {yN} "
-                                 f"(or a ring of {m})!")
+                                 f"(or a ring of {m}, or {half} half rows)!")
 
         keep = []
         for lo in range(0, len(accs), 64):

@@ -146,6 +146,7 @@ extern "C" int swiftly_b200_create(double W, int64_t N, int64_t xM, int64_t yN, 
     h->max_blocks = 0;
     for (int i = 0; i < 4; ++i) h->last_launch[i] = 0;
     h->last_cluster = 1;
+    h->n_fold_runs = 0;
     cudaError_t e = cudaMalloc((void**)&h->d_Fb, sizeof(double) * (size_t)(yN > 1 ? yN - 1 : 1));
     if (e == cudaSuccess) e = cudaMalloc((void**)&h->d_Fn, sizeof(double) * (size_t)h->m);
     if (e == cudaSuccess)
@@ -228,6 +229,15 @@ extern "C" void swiftly_b200_debug_last_launch(const swiftly_b200* h, int* out) 
 // when the 4 x Q form of extract_columns ran on two-CTA clusters, else 1)
 extern "C" int swiftly_b200_debug_last_cluster(const swiftly_b200* h) {
     return h ? h->last_cluster : 0;
+}
+
+// test hook: the runs of the last fold_column call into half-row accumulators, in launch order:
+// out[3 i .. 3 i + 2] = (first window row u, rows, pass 1 or 2); returns the number of runs (<= 8)
+extern "C" int swiftly_b200_debug_fold_runs(const swiftly_b200* h, int* out) {
+    if (!h) return 0;
+    if (out)
+        for (int i = 0; i < 3 * h->n_fold_runs; ++i) out[i] = h->fold_runs[i];
+    return h->n_fold_runs;
 }
 
 // ------------------------------------------------------------------ host staging
@@ -386,11 +396,20 @@ int window_copy_grid(const swiftly_b200* h, int64_t total) {
     Lines g = make_lines(sin, sout, in->n_lines);
 
 // ------------------------------------------------------------------ facet -> subgrid
+// real_half (always windowed): `in` holds doubles (strides counted in doubles), device arrays
+// only, and `out` receives the yN/2 + 1 half rows (PrepareFacetRealHalfOp)
 static int prepare_facet_impl(const swiftly_b200* h, const swiftly_b200_lines* in,
                               const swiftly_b200_lines* out, int64_t facet_off, bool windowed,
-                              void* stream) {
-    SW_PROLOGUE("prepare_facet", -1, h ? h->yN : -1, false)
+                              bool real_half, void* stream) {
+    if (real_half) {
+        if (!h) return einval("prepare_facet_real_half: NULL plan");
+        if (h->yN % 2) return einval("prepare_facet_real_half: yN_size must be even");
+        if (in && out && (in->location != SWIFTLY_B200_DEVICE || out->location != SWIFTLY_B200_DEVICE))
+            return einval("prepare_facet_real_half: device arrays only");
+    }
+    SW_PROLOGUE("prepare_facet", -1, h ? (real_half ? h->yN / 2 + 1 : h->yN) : -1, false)
     const int64_t yN = h->yN, fs = in->size;
+    const double* rin = real_half ? (const double*)in->data : nullptr;
     // windowed: line l of the output is additionally multiplied by Fb_c[l], the window the
     // NEXT prepare_facet (along the other axis) would apply to sample l of its lines
     const double* lw = nullptr;
@@ -435,7 +454,14 @@ static int prepare_facet_impl(const swiftly_b200* h, const swiftly_b200_lines* i
             a.shift_in = (int)pmod(fs / 2 - facet_off, yN);
             a.ncols = (int)nc;
             a.lw = lw ? lw + c0 : nullptr;
-            SW_TRY(run_prepare_facet_pass_a(h, a, s));
+            if (real_half) {
+                PrepareFacetPassARealOp ar;
+                static_cast<PrepareFacetPassAOp&>(ar) = a;
+                ar.rin = rin + c0;
+                SW_TRY(run_prepare_facet_pass_a_real(h, ar, s));
+            } else {
+                SW_TRY(run_prepare_facet_pass_a(h, a, s));
+            }
             PrepareFacetPassBOp b;
             b.g = g;
             b.g.in = scratch;
@@ -446,7 +472,13 @@ static int prepare_facet_impl(const swiftly_b200* h, const swiftly_b200_lines* i
             b.n2 = n2;
             b.ncols = (int)nc;
             b.scale = 1.0 / (double)yN;
-            SW_TRY(run_prepare_facet_pass_b(h, b, s));
+            if (real_half) {
+                PrepareFacetPassBHalfOp bh;
+                static_cast<PrepareFacetPassBOp&>(bh) = b;
+                SW_TRY(run_prepare_facet_pass_b_half(h, bh, s));
+            } else {
+                SW_TRY(run_prepare_facet_pass_b(h, b, s));
+            }
         }
         return stage_out(sout, s);
     }
@@ -462,14 +494,21 @@ static int prepare_facet_impl(const swiftly_b200* h, const swiftly_b200_lines* i
     op.rm_s_m = op.rm_base = 0;
     op.rm_mod = 1;
     op.lw = lw;
-    SW_TRY(run_prepare_facet(h, op, lines_adjacent(g), s));
+    if (real_half) {
+        PrepareFacetRealHalfOp rop;
+        static_cast<PrepareFacetOp&>(rop) = op;
+        rop.rin = rin;
+        SW_TRY(run_prepare_facet_real_half(h, rop, lines_adjacent(g), s));
+    } else {
+        SW_TRY(run_prepare_facet(h, op, lines_adjacent(g), s));
+    }
     return stage_out(sout, s);
 }
 
 extern "C" int swiftly_b200_prepare_facet(const swiftly_b200* h, const swiftly_b200_lines* in,
                                           const swiftly_b200_lines* out, int64_t facet_off,
                                           void* stream) {
-    return prepare_facet_impl(h, in, out, facet_off, false, stream);
+    return prepare_facet_impl(h, in, out, facet_off, false, false, stream);
 }
 
 // prepare_facet whose output lines are pre-multiplied by the Fb window of the other axis
@@ -478,7 +517,15 @@ extern "C" int swiftly_b200_prepare_facet_windowed(const swiftly_b200* h,
                                                    const swiftly_b200_lines* in,
                                                    const swiftly_b200_lines* out,
                                                    int64_t facet_off, void* stream) {
-    return prepare_facet_impl(h, in, out, facet_off, true, stream);
+    return prepare_facet_impl(h, in, out, facet_off, true, false, stream);
+}
+
+// prepare_facet_windowed of a real facet (doubles), only the half rows d <= yN/2 stored
+extern "C" int swiftly_b200_prepare_facet_real_half(const swiftly_b200* h,
+                                                    const swiftly_b200_lines* in,
+                                                    const swiftly_b200_lines* out,
+                                                    int64_t facet_off, void* stream) {
+    return prepare_facet_impl(h, in, out, facet_off, true, true, stream);
 }
 
 extern "C" int swiftly_b200_extract_from_facet(const swiftly_b200* h,
@@ -610,12 +657,13 @@ extern "C" int swiftly_b200_finish_facet(const swiftly_b200* h, const swiftly_b2
     return stage_out(sout, s);
 }
 
-extern "C" int swiftly_b200_finish_facet_real(const swiftly_b200* h,
-                                              const swiftly_b200_lines* in,
-                                              const swiftly_b200_lines* out, int64_t facet_off,
-                                              const double* mask, void* stream) {
+// half: `in` holds yN/2 + 1 half-row samples per line (FinishFacetRealHalfOp)
+static int finish_facet_real_impl(const swiftly_b200* h, const swiftly_b200_lines* in,
+                                  const swiftly_b200_lines* out, int64_t facet_off,
+                                  const double* mask, bool half, void* stream) {
     if (!h) return einval("finish_facet_real: NULL plan");
-    SW_TRY(check_lines(in, out, h->yN, -1, "finish_facet_real"));
+    if (half && h->yN % 2) return einval("finish_facet_real_half: yN_size must be even");
+    SW_TRY(check_lines(in, out, half ? h->yN / 2 + 1 : h->yN, -1, "finish_facet_real"));
     if (in->location != SWIFTLY_B200_DEVICE || out->location != SWIFTLY_B200_DEVICE)
         return einval("finish_facet_real: device arrays only");
     const int64_t yN = h->yN, fs = out->size;
@@ -641,6 +689,27 @@ extern "C" int swiftly_b200_finish_facet_real(const swiftly_b200* h,
     op.rout_ls = out->line_stride;
     op.rout_es = out->elem_stride;
     op.rmask = mask;
-    SW_TRY(run_finish_facet(h, op, lines_adjacent(op.g), s));
+    if (half) {
+        FinishFacetRealHalfOp hop;
+        static_cast<FinishFacetRealOp&>(hop) = op;
+        SW_TRY(run_finish_facet(h, hop, lines_adjacent(op.g), s));
+    } else {
+        SW_TRY(run_finish_facet(h, op, lines_adjacent(op.g), s));
+    }
     return SWIFTLY_B200_OK;
+}
+
+extern "C" int swiftly_b200_finish_facet_real(const swiftly_b200* h,
+                                              const swiftly_b200_lines* in,
+                                              const swiftly_b200_lines* out, int64_t facet_off,
+                                              const double* mask, void* stream) {
+    return finish_facet_real_impl(h, in, out, facet_off, mask, false, stream);
+}
+
+extern "C" int swiftly_b200_finish_facet_real_half(const swiftly_b200* h,
+                                                   const swiftly_b200_lines* in,
+                                                   const swiftly_b200_lines* out,
+                                                   int64_t facet_off, const double* mask,
+                                                   void* stream) {
+    return finish_facet_real_impl(h, in, out, facet_off, mask, true, stream);
 }

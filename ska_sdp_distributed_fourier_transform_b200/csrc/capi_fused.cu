@@ -266,9 +266,13 @@ static int extract_columns_impl(const swiftly_b200* h, int n_facets,
         return einval("extract_columns: between 1 and " + std::to_string(SW_MAX_COLUMN_FACETS) +
                       " facets per call");
     const int64_t yN = h->yN, m = h->m;
-    // whole prepared facets (yN rows) or row rings (m rows), the same for every facet of a call
-    const int64_t rows = bf_f[0].n_lines == m ? m : yN;
-    ExtractColumnsOp op;
+    // whole prepared facets (yN rows), row rings (m rows) or half rows of a real image (yN/2 + 1),
+    // the same for every facet of a call
+    const int64_t rows = bf_f[0].n_lines == m                          ? m
+                         : yN % 2 == 0 && bf_f[0].n_lines == yN / 2 + 1 ? yN / 2 + 1
+                                                                        : yN;
+    const bool half = rows != m && rows == yN / 2 + 1;
+    ExtractColumnsHalfOp op;
     for (int f = 0; f < n_facets; ++f) {
         const swiftly_b200_lines& i = bf_f[f];
         const swiftly_b200_lines& o = out[f];
@@ -276,7 +280,8 @@ static int extract_columns_impl(const swiftly_b200* h, int n_facets,
             return einval("extract_columns: device arrays only");
         if (i.n_lines != rows || i.elem_stride != 1 || o.elem_stride != 1)
             return einval("extract_columns: prepared facets must be yN_size (or, all of them, "
-                          "xM_yN_size ring) contiguous rows");
+                          "an xM_yN_size ring, or yN_size/2 + 1 half rows, yN_size even) "
+                          "contiguous rows");
         if (o.n_lines != m || o.size != yN)
             return einval("extract_columns: output must be xM_yN_size lines of yN_size samples");
         if (i.size > yN - 1) return einval("extract_columns: facet size must be at most yN_size - 1");
@@ -310,6 +315,7 @@ static int extract_columns_impl(const swiftly_b200* h, int n_facets,
         op.rm_s_m = (int)pmod(op.rm_s_m - op.rm_base, m);
         op.rm_base = 0;
     }
+    if (half) return run_extract_columns_half(h, op, false, (cudaStream_t)stream);
     return run_extract_columns(h, op, false, (cudaStream_t)stream);
 }
 
@@ -378,6 +384,54 @@ extern "C" int swiftly_b200_subgrid_to_facets(const swiftly_b200* h, int n_facet
     return run_subgrid_to_facets(h, op, false, (cudaStream_t)stream);
 }
 
+// fold_column into half-row accumulators.  Window row u (centred row base0 + u) goes to stored
+// row half_row(base0 + u); two rows of the window share a target when they are centred rows r and
+// -r (mod yN) -- a window across centred offset 0 or yN/2.  Pass 1 adds every row but the
+// conjugated member of such a pair, pass 2 those members, so that no launch has two lines with
+// one target (plain read-modify-write, no atomics: the sums are deterministic).  Each pass is
+// cut into runs of consecutive u, one launch each, in stream order.
+static int fold_column_half(const swiftly_b200* h, const FoldColumnOp& base, cudaStream_t s) {
+    const int n = base.n, m = base.lines_per;
+    auto second = [&](int u) {  // conjugated member of a shared target
+        bool cj;
+        const int i = half_row(wrap_add(base.base0, u, n), n, cj);
+        if (!cj) return false;
+        const int partner = wrap_sub(wrap_add(i, n / 2, n), base.base0, n);  // centred n/2 + i
+        return partner < m;
+    };
+    int runs[3 * 8];
+    int n_runs = 0;
+    for (int pass = 1; pass <= 2; ++pass) {
+        for (int u = 0; u < m;) {
+            if (second(u) != (pass == 2)) {
+                ++u;
+                continue;
+            }
+            int u1 = u + 1;
+            while (u1 < m && second(u1) == (pass == 2)) ++u1;
+            if (n_runs == 8) return einval("fold_column: window cut into more than 8 runs");
+            runs[3 * n_runs] = u;
+            runs[3 * n_runs + 1] = u1 - u;
+            runs[3 * n_runs + 2] = pass;
+            ++n_runs;
+            u = u1;
+        }
+    }
+    const int n_facets = (int)(base.g.n_lines / m);
+    for (int r = 0; r < n_runs; ++r) {
+        FoldColumnHalfOp op;
+        static_cast<FoldColumnOp&>(op) = base;
+        op.m = m;
+        op.u_lo = runs[3 * r];
+        op.lines_per = runs[3 * r + 1];
+        op.g.n_lines = (int64_t)n_facets * op.lines_per;
+        SW_TRY(run_fold_column_half(h, op, false, s));
+    }
+    for (int i = 0; i < 3 * n_runs; ++i) h->fold_runs[i] = runs[i];
+    h->n_fold_runs = n_runs;
+    return SWIFTLY_B200_OK;
+}
+
 // Fold one finished subgrid column into all facet accumulators (FoldColumnOp, kernels.cuh).
 extern "C" int swiftly_b200_fold_column(const swiftly_b200* h, int n_facets,
                                         const swiftly_b200_lines* accs,
@@ -389,8 +443,12 @@ extern "C" int swiftly_b200_fold_column(const swiftly_b200* h, int n_facets,
         return einval("fold_column: between 1 and " + std::to_string(SW_MAX_COLUMN_FACETS) +
                       " facets per call");
     const int64_t yN = h->yN, m = h->m;
-    // whole facet accumulators (yN rows) or row rings (m rows), the same for every facet
-    const int64_t rows = facet_accs[0].n_lines == m ? m : yN;
+    // whole facet accumulators (yN rows), row rings (m rows) or half rows of a real image
+    // (yN/2 + 1), the same for every facet
+    const int64_t rows = facet_accs[0].n_lines == m                          ? m
+                         : yN % 2 == 0 && facet_accs[0].n_lines == yN / 2 + 1 ? yN / 2 + 1
+                                                                             : yN;
+    const bool half = rows != m && rows == yN / 2 + 1;
     FoldColumnOp op;
     for (int f = 0; f < n_facets; ++f) {
         const swiftly_b200_lines& i = accs[f];
@@ -400,8 +458,9 @@ extern "C" int swiftly_b200_fold_column(const swiftly_b200* h, int n_facets,
         if (i.n_lines != m || i.size != yN || i.elem_stride != 1)
             return einval("fold_column: column accumulators must be xM_yN_size lines of yN_size");
         if (o.n_lines != rows || o.elem_stride != 1 || o.size > yN - 1)
-            return einval("fold_column: facet accumulators must be yN_size (or, all of them, "
-                          "xM_yN_size ring) lines of facet size");
+            return einval("fold_column: facet accumulators must be yN_size (or, all of them, an "
+                          "xM_yN_size ring, or yN_size/2 + 1 half rows, yN_size even) lines of "
+                          "facet size");
         FoldFacet& F = op.fac[f];
         F.in = (const cplx*)i.data;
         F.out = (cplx*)o.data;
@@ -428,5 +487,6 @@ extern "C" int swiftly_b200_fold_column(const swiftly_b200* h, int n_facets,
         op.s0_m = (int)pmod(op.s0_m - op.base0, m);
         op.base0 = 0;
     }
+    if (half) return fold_column_half(h, op, (cudaStream_t)stream);
     return run_fold_column(h, op, false, (cudaStream_t)stream);
 }

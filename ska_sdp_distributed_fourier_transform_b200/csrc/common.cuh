@@ -44,6 +44,14 @@ SW_HD cplx csub(cplx a, cplx b) { return mk(a.x - b.x, a.y - b.y); }
 SW_HD cplx cmul(cplx a, cplx b) { return mk(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 SW_HD cplx cscale(cplx a, double s) { return mk(a.x * s, a.y * s); }
 SW_HD cplx cconj(cplx a) { return mk(a.x, -a.y); }
+// a * b rounded on its own: never contracted with a following add into one fused multiply-add
+SW_HD double mul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
 // multiply by DIR * i   (DIR = -1: forward transform, +1: inverse transform)
 template <int DIR>
 SW_HD cplx mul_i(cplx a) {
@@ -70,6 +78,13 @@ SW_HD double ldg_d(const double* p) {
 // far larger than the 50 MB L2) should not push the few reused lines (twiddle / window
 // tables, split-kernel scratch) out of L2
 SW_HD cplx ld_stream(const cplx* p) {
+#if defined(__CUDA_ARCH__)
+    return __ldcs(p);
+#else
+    return *p;
+#endif
+}
+SW_HD double ld_stream_d(const double* p) {
 #if defined(__CUDA_ARCH__)
     return __ldcs(p);
 #else

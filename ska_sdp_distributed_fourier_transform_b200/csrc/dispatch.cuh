@@ -137,4 +137,33 @@ inline int unsupported(int n) {
     case 4096: return launch_lines<4096, DIR, Op>(h, op, lf, s);         \
     case 8192: return launch_lines<8192, DIR, Op>(h, op, lf, s);
 
+// The length dispatch of the facet-side line ops (op.n points, DIR = +1 inverse, -1 forward): one
+// CTA per line up to 8192, the 2 x 8192 split at 16384, split-F for F * 2^k; force_split (test
+// hook) runs the emulator's 128 and 512 as 2 x n/2.
+template <int DIR, class Op>
+int run_line_op(const swiftly_b200* h, const Op& op, bool lf, cudaStream_t s) {
+    const int n = op.n;
+    if (h->force_split && n >= 2 * MIN_FFT && n <= MAX_DIRECT_FFT) {
+        switch (n) {
+#if defined(SWIFTLY_EMU)
+            case 128: return launch_split<64, DIR, Op>(h, op, s);
+            case 512: return launch_split<256, DIR, Op>(h, op, s);
+#endif
+            default: break;
+        }
+    }
+    switch (n) {
+        SW_DIRECT_CASES(DIR, Op)
+        case 16384: return launch_split<8192, DIR, Op>(h, op, s);
+        default: break;
+    }
+    {
+        int M = 0, F = 0;
+        if (split_f_plan(n, &M, &F)) {
+            SW_SPLIT_F_CASES(DIR, Op, M, F)
+        }
+    }
+    return unsupported(n);
+}
+
 }  // namespace swiftly

@@ -8,10 +8,10 @@ namespace swiftly {
 
 // TMA-staged K2 (extract_tma.cuh): persistent CTAs, the facet row of the next line is copied
 // into shared memory by the bulk-copy engine while the current line is transformed
-template <int H, bool SPLIT>
+template <int H, bool SPLIT, bool HALF>
 static int launch_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op, int max_fs,
                               cudaStream_t s) {
-    typedef ExtractColumnsTmaKernel<H, SPLIT> K;
+    typedef ExtractColumnsTmaKernel<H, SPLIT, HALF> K;
     K k;
     static thread_local typename K::Maps maps;
     k.op = op;
@@ -65,8 +65,8 @@ static int launch_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op,
 // kernel code of swiftly_b200_debug_last_launch (plan.h)
 template <class K>
 struct K2Code;
-template <int Q>
-struct K2Code<ExtractColumnsTma4Kernel<Q>> {
+template <int Q, bool HALF>
+struct K2Code<ExtractColumnsTma4Kernel<Q, HALF>> {
     static const int value = LAUNCH_K2_TMA4;
 };
 template <int Q, bool BOTH>
@@ -150,10 +150,10 @@ static int launch_extract_tma4(const swiftly_b200* h, const ExtractColumnsOp& op
 // 4 x Q split on two-CTA clusters (extract_tma.cuh): the grid of the single-CTA form (one CTA per
 // SM, at most one per line, at most max_blocks), its CTAs paired.  Returns -1 when that grid is
 // odd or the device cannot hold all its clusters at once (then the single-CTA form runs on it).
-template <int Q>
+template <int Q, bool HALF>
 static int launch_extract_cluster(const swiftly_b200* h, const ExtractColumnsOp& op, int max_fs,
                                   cudaStream_t s) {
-    typedef ExtractColumnsClusterKernel<Q> K;
+    typedef ExtractColumnsClusterKernel<Q, HALF> K;
     K k;
     static thread_local typename K::Maps maps;
     k.op = op;
@@ -196,7 +196,10 @@ static bool pair_store_ok(const ExtractColumnsOp& op, int n_facets) {
     return true;
 }
 
-// returns -1 when the TMA-staged kernel does not apply (then the generic kernels run)
+// returns -1 when the TMA-staged kernel does not apply (then the generic kernels run).  HALF:
+// half rows (op.rows = yN/2 + 1) through the default forms only; the debug-selectable ones
+// (sg_variant 15, 17, 18, 19 and the emulator's force_split 3 .. 6) have no half instantiation
+template <bool HALF>
 static int try_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op, cudaStream_t s) {
     const int n = op.n;
     const int n_facets = (int)(op.g.n_lines / op.lines_per);
@@ -227,26 +230,26 @@ static int try_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op, cu
                     // (700 W), 8 facets of pre-windowed rows (tools/quick_k2.py): default 1.56 ms,
                     // 26: 2.19 (2.23 in an earlier session, with 17: 3.14, 18: 3.78, 19: 4.01,
                     // 15: 3.98).
-                    if (h->sg_variant == 17 && pair_store_ok(op, n_facets)) {
+                    if (!HALF && h->sg_variant == 17 && pair_store_ok(op, n_facets)) {
                         int rc = max_fs <= n / 2
                             ? launch_extract_park<4096, ExtractColumnsParkKernel<4096, 0>>(h, op, max_fs, s)
                             : launch_extract_park<4096, ExtractColumnsParkKernel<4096, 1>>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
-                    if (h->sg_variant == 18) {
+                    if (!HALF && h->sg_variant == 18) {
                         int rc = launch_extract_park<4096, ExtractColumnsParkKernel<4096, 2>>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
-                    if (h->sg_variant == 19) {
+                    if (!HALF && h->sg_variant == 19) {
                         int rc = launch_extract_park<4096, ExtractColumnsParkSkewKernel<4096>>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
-                    if (h->sg_variant != 15 && h->sg_variant != 26) {
-                        int rc = launch_extract_cluster<4096>(h, op, max_fs, s);
+                    if (HALF || (h->sg_variant != 15 && h->sg_variant != 26)) {
+                        int rc = launch_extract_cluster<4096, HALF>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
-                    int rc = h->sg_variant != 15
-                        ? launch_extract_tma4<4096, ExtractColumnsTma4Kernel<4096>>(h, op, max_fs, s, 4)
+                    int rc = HALF || h->sg_variant != 15
+                        ? launch_extract_tma4<4096, ExtractColumnsTma4Kernel<4096, HALF>>(h, op, max_fs, s, 4)
                         : (max_fs <= n / 2
                            ? launch_extract_tma4<4096, ExtractColumnsTmaDifKernel<4096, false>>(h, op, max_fs, s, 2)
                            : launch_extract_tma4<4096, ExtractColumnsTmaDifKernel<4096, true>>(h, op, max_fs, s, 2));
@@ -255,27 +258,27 @@ static int try_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op, cu
                 }
 #if defined(SWIFTLY_EMU)
                 case 512: {
-                    if (h->force_split == 4 && pair_store_ok(op, n_facets)) {
+                    if (!HALF && h->force_split == 4 && pair_store_ok(op, n_facets)) {
                         int rc = max_fs <= n / 2
                             ? launch_extract_park<128, ExtractColumnsParkKernel<128, 0>>(h, op, max_fs, s)
                             : launch_extract_park<128, ExtractColumnsParkKernel<128, 1>>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
-                    if (h->force_split == 5) {
+                    if (!HALF && h->force_split == 5) {
                         int rc = launch_extract_park<128, ExtractColumnsParkKernel<128, 2>>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
-                    if (h->force_split == 6) {
+                    if (!HALF && h->force_split == 6) {
                         int rc = launch_extract_park<128, ExtractColumnsParkSkewKernel<128>>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
                     // force_split 2: as the default at yN = 16384, 7: as sg_variant 26
                     if (h->force_split == 2) {
-                        int rc = launch_extract_cluster<128>(h, op, max_fs, s);
+                        int rc = launch_extract_cluster<128, HALF>(h, op, max_fs, s);
                         if (rc != -1) return rc;
                     }
-                    int rc = h->force_split != 3
-                        ? launch_extract_tma4<128, ExtractColumnsTma4Kernel<128>>(h, op, max_fs, s, 4)
+                    int rc = HALF || h->force_split != 3
+                        ? launch_extract_tma4<128, ExtractColumnsTma4Kernel<128, HALF>>(h, op, max_fs, s, 4)
                         : (max_fs <= n / 2
                            ? launch_extract_tma4<128, ExtractColumnsTmaDifKernel<128, false>>(h, op, max_fs, s, 2)
                            : launch_extract_tma4<128, ExtractColumnsTmaDifKernel<128, true>>(h, op, max_fs, s, 2));
@@ -287,55 +290,68 @@ static int try_extract_tma(const swiftly_b200* h, const ExtractColumnsOp& op, cu
             }
         }
         switch (n) {
-            case 16384: return launch_extract_tma<8192, true>(h, op, max_fs, s);
+            case 16384: return launch_extract_tma<8192, true, HALF>(h, op, max_fs, s);
 #if defined(SWIFTLY_EMU)
-            case 512: return launch_extract_tma<256, true>(h, op, max_fs, s);
+            case 512: return launch_extract_tma<256, true, HALF>(h, op, max_fs, s);
 #endif
             default: return -1;
         }
     }
     switch (n) {
 #if defined(SWIFTLY_EMU)
-        case 128: return launch_extract_tma<128, false>(h, op, max_fs, s);
-        case 512: return launch_extract_tma<512, false>(h, op, max_fs, s);
+        case 128: return launch_extract_tma<128, false, HALF>(h, op, max_fs, s);
+        case 512: return launch_extract_tma<512, false, HALF>(h, op, max_fs, s);
 #endif
-        case 1024: return launch_extract_tma<1024, false>(h, op, max_fs, s);
-        case 2048: return launch_extract_tma<2048, false>(h, op, max_fs, s);
-        case 4096: return launch_extract_tma<4096, false>(h, op, max_fs, s);
-        case 8192: return launch_extract_tma<8192, false>(h, op, max_fs, s);
+        case 1024: return launch_extract_tma<1024, false, HALF>(h, op, max_fs, s);
+        case 2048: return launch_extract_tma<2048, false, HALF>(h, op, max_fs, s);
+        case 4096: return launch_extract_tma<4096, false, HALF>(h, op, max_fs, s);
+        case 8192: return launch_extract_tma<8192, false, HALF>(h, op, max_fs, s);
         default: return -1;
     }
 }
 
-int run_extract_columns(const swiftly_b200* h, const ExtractColumnsOp& op, bool lf, cudaStream_t s) {
+// Op: ExtractColumnsOp, or ExtractColumnsHalfOp for half rows (no debug forms: sg_variant 3 and 4
+// do not apply to it either)
+template <class Op>
+static int run_extract_columns_op(const swiftly_b200* h, const Op& op, bool lf, cudaStream_t s) {
+    constexpr bool HALF = std::is_same<Op, ExtractColumnsHalfOp>::value;
     const int n = op.n;
-    if (h->sg_variant != 4 && h->sg_variant != 3) {  // 4: round-1 kernels (debug hook)
-        int rc = try_extract_tma(h, op, s);
+    if (HALF || (h->sg_variant != 4 && h->sg_variant != 3)) {  // 4: round-1 kernels (debug hook)
+        int rc = try_extract_tma<HALF>(h, op, s);
         if (rc != -1) return rc;
     }
     if (h->force_split && n >= 2 * MIN_FFT && n <= MAX_DIRECT_FFT) {
         switch (n) {
 #if defined(SWIFTLY_EMU)
-            case 128: return launch_split<64, +1, ExtractColumnsOp>(h, op, s);
-            case 512: return launch_split<256, +1, ExtractColumnsOp>(h, op, s);
+            case 128: return launch_split<64, +1, Op>(h, op, s);
+            case 512: return launch_split<256, +1, Op>(h, op, s);
 #endif
             default: break;
         }
     }
-    if (h->sg_variant == 3 && n == 16384)  // experiment: 4 x 4096 split, 256-thread CTAs
-        return launch_split_f<4096, +1, ExtractColumnsOp>(h, op, 4, s);
+    if (!HALF && h->sg_variant == 3 && n == 16384)  // experiment: 4 x 4096 split, 256-thread CTAs
+        return launch_split_f<4096, +1, Op>(h, op, 4, s);
     switch (n) {
-        SW_DIRECT_CASES(+1, ExtractColumnsOp)
-        case 16384: return launch_split<8192, +1, ExtractColumnsOp>(h, op, s);
+        SW_DIRECT_CASES(+1, Op)
+        case 16384: return launch_split<8192, +1, Op>(h, op, s);
         default: break;
     }
     {
         int M = 0, F = 0;
         if (split_f_plan(n, &M, &F)) {
-            SW_SPLIT_F_CASES(+1, ExtractColumnsOp, M, F)
+            SW_SPLIT_F_CASES(+1, Op, M, F)
         }
     }
     return unsupported(n);
+}
+
+int run_extract_columns(const swiftly_b200* h, const ExtractColumnsOp& op, bool lf, cudaStream_t s) {
+    return run_extract_columns_op(h, op, lf, s);
+}
+
+int run_extract_columns_half(const swiftly_b200* h, const ExtractColumnsHalfOp& op, bool lf,
+                             cudaStream_t s) {
+    return run_extract_columns_op(h, op, lf, s);
 }
 
 }  // namespace swiftly

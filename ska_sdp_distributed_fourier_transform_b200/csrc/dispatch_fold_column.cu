@@ -5,28 +5,7 @@
 namespace swiftly {
 
 int run_fold_column(const swiftly_b200* h, const FoldColumnOp& op, bool lf, cudaStream_t s) {
-    const int n = op.n;
-    if (h->force_split && n >= 2 * MIN_FFT && n <= MAX_DIRECT_FFT) {
-        switch (n) {
-#if defined(SWIFTLY_EMU)
-            case 128: return launch_split<64, -1, FoldColumnOp>(h, op, s);
-            case 512: return launch_split<256, -1, FoldColumnOp>(h, op, s);
-#endif
-            default: break;
-        }
-    }
-    switch (n) {
-        SW_DIRECT_CASES(-1, FoldColumnOp)
-        case 16384: return launch_split<8192, -1, FoldColumnOp>(h, op, s);
-        default: break;
-    }
-    {
-        int M = 0, F = 0;
-        if (split_f_plan(n, &M, &F)) {
-            SW_SPLIT_F_CASES(-1, FoldColumnOp, M, F)
-        }
-    }
-    return unsupported(n);
+    return run_line_op<-1>(h, op, lf, s);
 }
 
 }  // namespace swiftly

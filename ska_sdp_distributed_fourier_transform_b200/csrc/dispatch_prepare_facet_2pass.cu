@@ -22,4 +22,15 @@ int run_prepare_facet_pass_b(const swiftly_b200* h, const PrepareFacetPassBOp& o
     SW_2PASS_CASES(PrepareFacetPassBOp, op.n2)
 }
 
+// real facet into half rows (real images)
+int run_prepare_facet_pass_a_real(const swiftly_b200* h, const PrepareFacetPassARealOp& op,
+                                  cudaStream_t s) {
+    SW_2PASS_CASES(PrepareFacetPassARealOp, op.n1)
+}
+
+int run_prepare_facet_pass_b_half(const swiftly_b200* h, const PrepareFacetPassBHalfOp& op,
+                                  cudaStream_t s) {
+    SW_2PASS_CASES(PrepareFacetPassBHalfOp, op.n2)
+}
+
 }  // namespace swiftly

@@ -28,13 +28,18 @@ namespace swiftly {
 // pieces of at most 64 KiB.  Shared by all TMA-staged K2 kernels.
 // PAIR: the row goes to the same offsets in both CTAs of a two-CTA cluster (multicast); the
 // issuing thread, of either CTA, arms both CTAs' barriers.
-template <class Maps, bool PAIR = false, class Ctx>
+// HALF: the rows are half rows (include/swiftly_b200.h): the window row's stored row is fetched.
+template <class Maps, bool PAIR = false, bool HALF = false, class Ctx>
 SW_HD void k2_issue_row(const Ctx& ctx, const ExtractColumnsOp& op, int swizzled, int box_chunks,
                         cplx* in, uint64_t* bar, int64_t line) {
     const int f = (int)(line / op.lines_per);
     const int l = (int)(line - (int64_t)f * op.lines_per);
     const ColumnFacet& F = op.fac[f];
-    const int64_t row = wrap_add(op.rm_base, wrap_sub(l, op.rm_s_m, op.lines_per), op.n);
+    int64_t row = wrap_add(op.rm_base, wrap_sub(l, op.rm_s_m, op.lines_per), op.n);
+    if constexpr (HALF) {
+        bool cj;
+        row = half_row((int)row, op.n, cj);
+    }
     auto expect = [&](uint32_t bytes) {
         if constexpr (PAIR) {
             ctx.tx_expect_peer(bar, 0, bytes);
@@ -68,7 +73,9 @@ SW_HD void k2_issue_row(const Ctx& ctx, const ExtractColumnsOp& op, int swizzled
     }
 }
 
-template <int H, bool SPLIT>
+// HALF (every TMA form the default dispatch runs): the rows are half rows; a line whose window
+// row is stored conjugated negates the imaginary part of every staged sample it reads.
+template <int H, bool SPLIT, bool HALF = false>
 struct ExtractColumnsTmaKernel {
     static constexpr int DIR = +1;
     static constexpr int T = FftCfg<H>::T;
@@ -115,7 +122,7 @@ struct ExtractColumnsTmaKernel {
 
     template <class Ctx>
     SW_HD void issue(const Ctx& ctx, cplx* in, uint64_t* bar, int64_t line) const {
-        k2_issue_row<Maps>(ctx, op, swizzled, box_chunks, in, bar, line);
+        k2_issue_row<Maps, false, HALF>(ctx, op, swizzled, box_chunks, in, bar, line);
     }
 
     template <class Ctx>
@@ -142,11 +149,18 @@ struct ExtractColumnsTmaKernel {
             const double scale = op.scale;
             const bool swz = swizzled != 0;
             // natural-order input sample q of the zero-padded, rotated, Fb-weighted row
+            bool cj = false;
+            if constexpr (HALF) half_row(wrap_add(op.rm_base, wrap_sub(l, op.rm_s_m, op.lines_per), n), n, cj);
             auto sample = [&](int q) {
                 int k = wrap_add(q, shift_in, n);
                 if (k >= fs) return mk(0.0, 0.0);
                 const int ks = swz ? ((k & ~7) | ((k ^ (k >> 3)) & 7)) : k;
-                return fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                if constexpr (HALF) {
+                    const cplx x = fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                    return cj ? cconj(x) : x;
+                } else {
+                    return fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                }
             };
             auto put = [&](int p, cplx v) {
                 int pc = wrap_add(p, n / 2, n);
@@ -217,7 +231,7 @@ struct ExtractColumnsTmaKernel {
 // stride-4 reads of the staged row are conflict free thanks to the 128-byte swizzle.  All
 // four t_q are parked in a per-CTA scratch (L2 resident); after a CTA barrier every thread
 // combines its share of the k range and writes four unit-stride output streams.
-template <int Q>
+template <int Q, bool HALF = false>
 struct ExtractColumnsTma4Kernel {
     static constexpr int DIR = +1;
     static constexpr int TG = FftCfg<Q>::T;  // threads per group
@@ -248,7 +262,7 @@ struct ExtractColumnsTma4Kernel {
 
     template <class Ctx>
     SW_HD void issue(const Ctx& ctx, cplx* in, uint64_t* bar, int64_t line) const {
-        k2_issue_row<Maps>(ctx, op, swizzled, box_chunks, in, bar, line);
+        k2_issue_row<Maps, false, HALF>(ctx, op, swizzled, box_chunks, in, bar, line);
     }
 
     // group barrier; after the first-pass loads of the group's LAST sub-transform the staging
@@ -307,11 +321,18 @@ struct ExtractColumnsTma4Kernel {
             cplx* o = F.out + (int64_t)l * F.out_ls;
             const double scale = op.scale;
             const bool swz = swizzled != 0;
+            bool cj = false;
+            if constexpr (HALF) half_row(wrap_add(op.rm_base, wrap_sub(l, op.rm_s_m, op.lines_per), n), n, cj);
             auto sample = [&](int q) {
                 int k = wrap_add(q, shift_in, n);
                 if (k >= fs) return mk(0.0, 0.0);
                 const int ks = swz ? ((k & ~7) | ((k ^ (k >> 3)) & 7)) : k;
-                return fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                if constexpr (HALF) {
+                    const cplx x = fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                    return cj ? cconj(x) : x;
+                } else {
+                    return fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                }
             };
             ctx.tx_wait(bar, parity);
             parity ^= 1;
@@ -386,7 +407,7 @@ struct ExtractColumnsTma4Kernel {
 // Same operations in the same order as ExtractColumnsTma4Kernel, so the same bits.  The staging
 // buffer is dead once all four groups of the pair have done their first-pass loads: the last of
 // them to get there issues the next row (counter in CTA 0).
-template <int Q>
+template <int Q, bool HALF = false>
 struct ExtractColumnsClusterKernel {
     static constexpr int DIR = +1;
     static constexpr int CLUSTER = 2;
@@ -419,7 +440,7 @@ struct ExtractColumnsClusterKernel {
 
     template <class Ctx>
     SW_HD void issue(const Ctx& ctx, cplx* in, uint64_t* bar, int64_t line) const {
-        k2_issue_row<Maps, true>(ctx, op, swizzled, box_chunks, in, bar, line);
+        k2_issue_row<Maps, true, HALF>(ctx, op, swizzled, box_chunks, in, bar, line);
     }
 
     template <class Ctx>
@@ -477,11 +498,18 @@ struct ExtractColumnsClusterKernel {
             cplx* o = F.out + (int64_t)l * F.out_ls;
             const double scale = op.scale;
             const bool swz = swizzled != 0;
+            bool cj = false;
+            if constexpr (HALF) half_row(wrap_add(op.rm_base, wrap_sub(l, op.rm_s_m, op.lines_per), n), n, cj);
             auto sample = [&](int q) {
                 int k = wrap_add(q, shift_in, n);
                 if (k >= fs) return mk(0.0, 0.0);
                 const int ks = swz ? ((k & ~7) | ((k ^ (k >> 3)) & 7)) : k;
-                return fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                if constexpr (HALF) {
+                    const cplx x = fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                    return cj ? cconj(x) : x;
+                } else {
+                    return fb ? cscale(in[ks], ldg_d(fb + k)) : in[ks];
+                }
             };
             ctx.tx_wait(bar, parity);
             parity ^= 1;

@@ -35,6 +35,15 @@ SW_HD int wrap_sub(int a, int b, int n) {  // (a - b) mod n for 0 <= a,b < n
     return r < 0 ? r + n : r;
 }
 
+// Half rows of a real image (include/swiftly_b200.h, "Half rows"): stored row d, 0 <= d <= n/2,
+// holds centred row (n/2 + d) mod n, i.e. natural FFT index d.  Centred row r is stored row
+// half_row(r, n, conj), conjugated when `conj` is set (rows n/2 + d and n/2 - d are conjugates).
+SW_HD int half_row(int r, int n, bool& conj) {
+    const int d = wrap_sub(r, n / 2, n);
+    conj = d > n / 2;
+    return conj ? n - d : d;
+}
+
 // ------------------------------------------------------------------ ops
 // prepare_facet (core.py:189-222): out = ifft_c(roll(pad_mid(facet * Fb_c, yN), facet_off))
 struct PrepareFacetOp {
@@ -69,6 +78,29 @@ struct PrepareFacetOp {
         int64_t row = rm_m ? (int64_t)wrap_add(rm_base, wrap_sub((int)line, rm_s_m, rm_m), rm_mod)
                            : line;
         prefetch_l2(g.in + row * g.in_ls + (int64_t)k * g.in_es);
+    }
+};
+
+// prepare_facet of a REAL facet into half rows: the input samples are doubles (`rin`, strides
+// g.in_ls / g.in_es counted in doubles; no row map) and only the outputs at natural index
+// p <= n/2 are stored, at row p.  A real sample x enters as (x * Fb, 0 * Fb), the product the
+// complex op forms on the promoted sample, so the stored rows are bitwise those of PrepareFacetOp.
+struct PrepareFacetRealHalfOp : PrepareFacetOp {
+    const double* rin;
+    SW_HD cplx load(int64_t line, int q) const {
+        int k = wrap_add(q, shift_in, n);
+        if (k >= fs) return mk(0.0, 0.0);
+        const double f = ldg_d(fb + k);
+        return mk(ld_stream_d(rin + line * g.in_ls + (int64_t)k * g.in_es) * f, 0.0 * f);
+    }
+    SW_HD void store(int64_t line, int p, cplx v) const {
+        if (p > n / 2) return;
+        const double f = lw ? scale * ldg_d(lw + line) : scale;
+        st_stream(g.out + line * g.out_ls + (int64_t)p * g.out_es, cscale(v, f));
+    }
+    SW_HD void prefetch(int64_t line, int q) const {
+        int k = wrap_add(q, shift_in, n);
+        if (k < fs) prefetch_l2(rin + line * g.in_ls + (int64_t)k * g.in_es);
     }
 };
 
@@ -146,6 +178,30 @@ struct PrepareFacetPassBOp {
         st_stream(g.out + (int64_t)pc * g.out_es + c, cscale(v, scale));
     }
 };
+// The two passes for a REAL facet into half rows: pass A reads doubles (`rin`, row stride
+// g.in_es doubles) as PrepareFacetRealHalfOp does, the scratch T stays full size; pass B stores
+// natural index d = k1 + n1 k2 at row d when d <= n/2 and drops the other rows.
+struct PrepareFacetPassARealOp : PrepareFacetPassAOp {
+    const double* rin;
+    SW_HD cplx load(int64_t line, int q) const {
+        const int j2 = (int)(line / ncols);
+        const int c = (int)(line - (int64_t)j2 * ncols);
+        int k = wrap_add(q * n2 + j2, shift_in, n);
+        if (k >= fs) return mk(0.0, 0.0);
+        double f = ldg_d(fb + k);
+        if (lw) f *= ldg_d(lw + c);
+        return mk(ld_stream_d(rin + (int64_t)k * g.in_es + c) * f, 0.0 * f);
+    }
+};
+struct PrepareFacetPassBHalfOp : PrepareFacetPassBOp {
+    SW_HD void store(int64_t line, int k2, cplx v) const {
+        const int k1 = (int)(line / ncols);
+        const int c = (int)(line - (int64_t)k1 * ncols);
+        const int d = k1 + n1 * k2;
+        if (d > n / 2) return;
+        st_stream(g.out + (int64_t)d * g.out_es + c, cscale(v, scale));
+    }
+};
 
 // Several prepare_facet jobs with a row map (extract_column of MANY facets, one launch):
 // global line L = f * lines_per + l belongs to facet f; per-facet base pointers / shifts
@@ -191,6 +247,32 @@ struct ExtractColumnsOp {
         int k = wrap_add(q, F.shift_in, n);
         if (k >= F.fs) return;
         int64_t row = wrap_add(rm_base, wrap_sub(l, rm_s_m, lines_per), n);
+        prefetch_l2(F.in + row * F.in_ls + k);
+    }
+};
+// ExtractColumnsOp on half rows (rows = n/2 + 1): window row r is read from stored row
+// half_row(r) and conjugated when that says so -- bitwise the load of the full Hermitian rows
+struct ExtractColumnsHalfOp : ExtractColumnsOp {
+    SW_HD cplx load(int64_t line, int q) const {
+        const int f = (int)(line / lines_per);
+        const int l = (int)(line - (int64_t)f * lines_per);
+        const ColumnFacet& F = fac[f];
+        int k = wrap_add(q, F.shift_in, n);
+        if (k >= F.fs) return mk(0.0, 0.0);
+        bool cj;
+        const int64_t row = half_row(wrap_add(rm_base, wrap_sub(l, rm_s_m, lines_per), n), n, cj);
+        cplx x = ld_stream(F.in + row * F.in_ls + k);
+        if (fb) x = cscale(x, ldg_d(fb + F.fb_off + k));
+        return cj ? cconj(x) : x;
+    }
+    SW_HD void prefetch(int64_t line, int q) const {
+        const int f = (int)(line / lines_per);
+        const int l = (int)(line - (int64_t)f * lines_per);
+        const ColumnFacet& F = fac[f];
+        int k = wrap_add(q, F.shift_in, n);
+        if (k >= F.fs) return;
+        bool cj;
+        const int64_t row = half_row(wrap_add(rm_base, wrap_sub(l, rm_s_m, lines_per), n), n, cj);
         prefetch_l2(F.in + row * F.in_ls + k);
     }
 };
@@ -276,6 +358,40 @@ struct FoldColumnOp {
         *o = mk(a.x + w * v.x, a.y + w * v.y);
     }
 };
+// FoldColumnOp into half-row facet accumulators, for the run of window rows u in
+// [u_lo, u_lo + lines_per) (u = (t - s0_m) mod m, t the column accumulator row).  Row
+// base0 + u goes to stored row half_row(.): conj(w v) is added where that flags a conjugate,
+// w v elsewhere.  The host cuts the window into runs whose rows have distinct targets.  The
+// conjugated add rounds the product first (no fused multiply-add), so that one fold into zeroed
+// accumulators is bitwise x[d] + conj(x[-d]) of the full-row fold x; the plain add is the
+// full-row op's.
+struct FoldColumnHalfOp : FoldColumnOp {
+    int m, u_lo;
+    SW_HD cplx load(int64_t line, int q) const {
+        const int f = (int)(line / lines_per);
+        const int j = (int)(line - (int64_t)f * lines_per);
+        const FoldFacet& F = fac[f];
+        const int t = wrap_add(u_lo + j, s0_m, m);
+        int qc = wrap_add(q, n / 2, n);
+        return ld_stream(F.in + (int64_t)t * F.in_ls + qc);
+    }
+    SW_HD void store(int64_t line, int p, cplx v) const {
+        const int f = (int)(line / lines_per);
+        const int j = (int)(line - (int64_t)f * lines_per);
+        const FoldFacet& F = fac[f];
+        int pc = wrap_add(p, n / 2, n);
+        int k = wrap_sub(pc, F.start1, n);
+        if (k >= F.fs) return;
+        double w = ldg_d(fb + F.fb_off + k);
+        if (F.mask) w *= ldg_d(F.mask + k);
+        bool cj;
+        const int64_t row = half_row(wrap_add(base0, u_lo + j, n), n, cj);
+        cplx* o = F.out + row * F.out_ls + k;
+        cplx a = *o;
+        *o = cj ? mk(a.x + mul_rn(w, v.x), a.y - mul_rn(w, v.y))
+                : mk(a.x + w * v.x, a.y + w * v.y);
+    }
+};
 
 // finish_facet (core.py:452-484): out[k] = Fb_c[k] * fft_c(sum)[(yN/2 - fs//2 + k + off) mod yN]
 struct FinishFacetOp {
@@ -318,6 +434,22 @@ struct FinishFacetRealOp : FinishFacetOp {
             if (rmask) x *= ldg_d(rmask + k);
             st_stream_d(rout + line * rout_ls + (int64_t)k * rout_es, x);
         }
+    }
+};
+
+// FinishFacetRealOp reading half-row lines (n/2 + 1 samples, natural order): the loader forms the
+// Hermitian part of the full line, whose transform has the same real part,
+//   0.5 H[q] (0 < q < n/2),  0.5 conj(H[n - q]) (q > n/2),  (Re H[q], 0) (q = 0, n/2)
+struct FinishFacetRealHalfOp : FinishFacetRealOp {
+    SW_HD cplx load(int64_t line, int q) const {
+        const cplx* p = g.in + line * g.in_ls;
+        if (q == 0 || q == n / 2) return mk(ld_stream(p + (int64_t)q * g.in_es).x, 0.0);
+        if (q < n / 2) return cscale(ld_stream(p + (int64_t)q * g.in_es), 0.5);
+        const cplx x = ld_stream(p + (int64_t)(n - q) * g.in_es);
+        return mk(0.5 * x.x, -(0.5 * x.y));
+    }
+    SW_HD void prefetch(int64_t line, int q) const {
+        prefetch_l2(g.in + line * g.in_ls + (int64_t)(q <= n / 2 ? q : n - q) * g.in_es);
     }
 };
 

@@ -29,6 +29,10 @@ struct swiftly_b200 {
     // line-fastest flag or staging capacity, grid), see swiftly_b200_debug_last_launch
     mutable int last_launch[4];
     mutable int last_cluster;  // CTAs per cluster of that launch (swiftly_b200_debug_last_cluster)
+    // debug / test: the runs of the last fold_column call into half-row accumulators, (first
+    // window row u, rows, pass) each, in launch order (swiftly_b200_debug_fold_runs)
+    mutable int fold_runs[3 * 8];
+    mutable int n_fold_runs;
 };
 
 namespace swiftly {
@@ -87,7 +91,7 @@ inline bool is_pow2(int64_t n) { return n > 0 && (n & (n - 1)) == 0; }
 // dispatchers, one translation unit each (compile time!): launch `op` over all
 // its lines with an n-point transform.  dir = -1 forward, +1 inverse.
 int run_prepare_facet(const swiftly_b200* h, const PrepareFacetOp& op, bool line_fastest, cudaStream_t s);
-// FinishFacetOp or FinishFacetRealOp (dispatch_finish_facet.cuh)
+// FinishFacetOp, FinishFacetRealOp or FinishFacetRealHalfOp (dispatch_finish_facet.cuh)
 template <class Op>
 int run_finish_facet(const swiftly_b200* h, const Op& op, bool line_fastest, cudaStream_t s);
 int run_add_to_subgrid(const swiftly_b200* h, const AddToSubgridOp& op, bool line_fastest, cudaStream_t s);
@@ -99,6 +103,13 @@ int run_prepare_facet_pass_b(const swiftly_b200* h, const PrepareFacetPassBOp& o
 int run_subgrid_to_facets(const swiftly_b200* h, const SubgridToFacetsOp& op, bool line_fastest, cudaStream_t s);
 int run_fold_column(const swiftly_b200* h, const FoldColumnOp& op, bool line_fastest, cudaStream_t s);
 int run_extract_columns(const swiftly_b200* h, const ExtractColumnsOp& op, bool line_fastest, cudaStream_t s);
+// half rows of real images (include/swiftly_b200.h, "Half rows"); FinishFacetRealHalfOp goes
+// through run_finish_facet
+int run_prepare_facet_real_half(const swiftly_b200* h, const PrepareFacetRealHalfOp& op, bool line_fastest, cudaStream_t s);
+int run_prepare_facet_pass_a_real(const swiftly_b200* h, const PrepareFacetPassARealOp& op, cudaStream_t s);
+int run_prepare_facet_pass_b_half(const swiftly_b200* h, const PrepareFacetPassBHalfOp& op, cudaStream_t s);
+int run_extract_columns_half(const swiftly_b200* h, const ExtractColumnsHalfOp& op, bool line_fastest, cudaStream_t s);
+int run_fold_column_half(const swiftly_b200* h, const FoldColumnHalfOp& op, bool line_fastest, cudaStream_t s);
 
 // fused subgrid axis kernel (dispatch_subgrid_axis.cu); `k` carries everything but the tables
 struct SubgridAxisArgs {
