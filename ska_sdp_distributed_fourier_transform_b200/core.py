@@ -15,6 +15,10 @@ Arrays may be
   * ``torch.Tensor`` on a CUDA device (complex128): used in place on the
     current torch stream, results are device tensors -- the fast path used by
     ``SwiftlyForward`` / ``SwiftlyBackward``.
+
+Masks (0/1 sample weights, or None) may be numpy arrays or tensors of any float dtype on any
+device: each is converted to a contiguous float64 array where the call's output lives, and must
+have as many samples as the output has along the axis it masks (``ValueError`` otherwise).
 """
 
 import ctypes
@@ -59,54 +63,72 @@ class PreparedSumFinish:
         self.core = core
         self.axis = axis
         self.n_groups = len(groups)
-        other = 1 - axis
-        flat = [s for grp in groups for s in grp]
-        self._keep = [t for t, _ in flat]  # the sources must outlive the block
-        self._arr = (_lib.Source * max(1, len(flat)))()
-        for i, (t, facet_off) in enumerate(flat):
-            core._check_tensor(t)
-            if t.dtype != torch.complex128 or t.dim() != 2:
-                raise ValueError("sources must be 2-D complex128 device tensors")
-            if t.shape[other] != n_lines:
-                raise ValueError(f"source has {t.shape[other]} lines, output {n_lines}")
-            self._arr[i] = _lib.Source(t.data_ptr(), t.stride(other), t.stride(axis),
-                                       t.shape[axis], int(facet_off))
-        self._sizes = (ctypes.c_int32 * self.n_groups)(*[len(g) for g in groups])
+        # (the sources must outlive the block)
+        self._arr, self._sizes, self._keep = core._sources(groups, axis, n_lines)
         self._offs = (ctypes.c_int64 * self.n_groups)()
         self._mptrs = (ctypes.c_void_p * self.n_groups)()
         self._optrs = (ctypes.c_void_p * self.n_groups)()
         self._dout = _lib.Lines(0, int(n_lines), int(size), int(out_strides[0]),
                                 int(out_strides[1]), _lib.DEVICE)
-        self._device = flat[0][0].device if flat else None
+        # shape and strides of one group's output tensor, whose lines run along the other axis
+        step = 1 if axis == 1 else -1
+        self._shape = (int(n_lines), int(size))[::step]
+        self._strides = (int(out_strides[0]), int(out_strides[1]))[::step]
+
+    def _check_out(self, o, k=0):
+        """``o`` (after its first ``k`` dimensions) must be a group's output."""
+        self.core._check_tensor(o)
+        shape, strides = tuple(o.shape)[k:], o.stride()[k:]
+        if o.dtype != torch.complex128 or shape != self._shape or strides != self._strides:
+            raise ValueError(f"output has shape {shape}, strides {strides} and dtype {o.dtype}; "
+                             f"the block writes {self._shape}, strides {self._strides}, "
+                             f"complex128")
 
     def launch(self, subgrid_offs, masks=None, out=None, out_group_stride=0, outs=None,
                n_groups=None, out_ptrs=None, stream_of=None):
         """Launch for the first ``n_groups`` groups (default: all).
 
         :param subgrid_offs: one offset per group
-        :param masks: None or one float64 device tensor / None per group
-        :param out, out_group_stride: base tensor of group 0 and the stride between groups, or
+        :param masks: None or one mask / None per group of the block's ``size`` samples (a mask
+            object repeated for consecutive groups is converted once)
+        :param out, out_group_stride: group 0's output, or the outputs of all groups stacked
+            along a leading axis of stride ``out_group_stride``, or
         :param outs: one output tensor per group (same shape / strides, different buffers), or
-        :param out_ptrs: their device addresses (ints) with ``stream_of`` a tensor on the device
+        :param out_ptrs: their device addresses (ints) with ``stream_of`` a tensor on the device.
+            Raw addresses cannot be checked: each must hold a group's output with the shape and
+            strides given to :meth:`SwiftlyCoreB200.prepare_sum_finish`
         """
         n = self.n_groups if n_groups is None else int(n_groups)
         core = self.core
+        if out_ptrs is not None:
+            core._check_tensor(stream_of)
+            like = stream_of
+        elif outs is not None:
+            if len(outs) < n:
+                raise ValueError(f"{len(outs)} outputs for {n} groups")
+            for o in outs[:n]:
+                self._check_out(o)
+            like, out_ptrs = outs[0], [o.data_ptr() for o in outs]
+        else:
+            k = 1 if out.dim() == 3 else 0  # the outputs of all groups stacked
+            if n > (out.shape[0] if k else 1) or (k and out.stride(0) != out_group_stride):
+                raise ValueError(f"out of shape {tuple(out.shape)} and strides {out.stride()} "
+                                 f"does not hold {n} groups {out_group_stride} samples apart")
+            self._check_out(out, k)
+            like = out
+        keep, prev, ptr = [], (), None
         for g in range(n):
             self._offs[g] = int(subgrid_offs[g])
             mk = None if masks is None else masks[g]
-            self._mptrs[g] = None if mk is None else mk.data_ptr()
-        if outs is not None or out_ptrs is not None:
-            if out_ptrs is not None:
-                for g in range(n):
-                    self._optrs[g] = out_ptrs[g]
-                stream = core._stream(stream_of)
-            else:
-                for g in range(n):
-                    self._optrs[g] = outs[g].data_ptr()
-                stream = core._stream(outs[0])
+            if mk is not prev:  # the drivers pass one mask object for many groups
+                prev, ptr = mk, core._mask_ptr(mk, like, self._dout.size, keep)
+            self._mptrs[g] = ptr
+        if out is None:
+            for g in range(n):
+                self._optrs[g] = out_ptrs[g]
             rc = core._lib.swiftly_b200_sum_finish_axis_scattered(
                 core._plan, self._arr, self._sizes, n, ctypes.byref(self._dout), self._optrs,
-                self._offs, self._mptrs, stream)
+                self._offs, self._mptrs, core._stream(like))
         else:
             self._dout.data = out.data_ptr()
             rc = core._lib.swiftly_b200_sum_finish_axis_batched(
@@ -261,19 +283,42 @@ class SwiftlyCoreB200:
                 f"tensor is on cuda:{t.device.index}, the plan on cuda:{self.device}"
             )
 
-    def _mask_ptr(self, mask, like, keep):
-        """Pointer to a float64 mask living where ``like`` lives (or NULL)."""
+    @staticmethod
+    def _mask_ptr(mask, like, size, keep, what="subgrid"):
+        """Address of ``mask`` (None: NULL) converted to a contiguous float64 array living where
+        ``like`` lives; it must have ``size`` samples.  The converted mask is appended to
+        ``keep``, which the caller holds until the C call returns."""
         if mask is None:
-            return ctypes.c_void_p(0)
+            return None
         if _is_tensor(like):
             if not _is_tensor(mask):
                 mask = torch.as_tensor(numpy.asarray(mask, dtype=float), device=like.device)
-            mask = mask.to(torch.float64).contiguous()
-            keep.append(mask)
-            return ctypes.c_void_p(mask.data_ptr())
-        mask = numpy.ascontiguousarray(mask, dtype=float)
+            mask = mask.to(like.device, torch.float64).contiguous()
+            n, ptr = mask.numel(), mask.data_ptr()
+        else:
+            mask = numpy.ascontiguousarray(mask.cpu() if _is_tensor(mask) else mask, dtype=float)
+            n, ptr = mask.size, mask.ctypes.data
+        if n != size:
+            raise ValueError(f"mask must have the {what} size")
         keep.append(mask)
-        return ctypes.c_void_p(mask.ctypes.data)
+        return ptr
+
+    def _sources(self, groups, axis, n_lines):
+        """``Source`` array, int32 group sizes and source tensors (to keep alive) of ``groups``,
+        lists of ``(tensor, facet_off)`` read along ``axis`` into outputs of ``n_lines`` lines."""
+        other = 1 - axis
+        flat = [s for grp in groups for s in grp]
+        arr = (_lib.Source * max(1, len(flat)))()
+        for i, (t, facet_off) in enumerate(flat):
+            self._check_tensor(t)
+            if t.dtype != torch.complex128 or t.dim() != 2:
+                raise ValueError("sources must be 2-D complex128 device tensors")
+            if t.shape[other] != n_lines:
+                raise ValueError(f"source has {t.shape[other]} lines, output {n_lines}")
+            arr[i] = _lib.Source(t.data_ptr(), t.stride(other), t.stride(axis), t.shape[axis],
+                                 int(facet_off))
+        sizes = (ctypes.c_int32 * len(groups))(*[len(g) for g in groups])
+        return arr, sizes, [t for t, _ in flat]
 
     def _run(self, fn_name, in_arr, out_size, axis, out, offset, accumulate=False, mask=None):
         """Shape handling shared by all primitives.
@@ -320,7 +365,8 @@ class SwiftlyCoreB200:
         keep = []
         args = [self._plan, ctypes.byref(din), ctypes.byref(dout), int(offset)]
         if fn_name in ("swiftly_b200_finish_subgrid", "swiftly_b200_finish_facet"):
-            args.append(self._mask_ptr(mask, out, keep))
+            what = fn_name.rsplit("_", 1)[1]  # "subgrid" / "facet"
+            args.append(self._mask_ptr(mask, out, shape[axis], keep, what))
         args.append(self._stream(in_arr))
         rc = getattr(self._lib, fn_name)(*args)
         _lib.check(self._lib, rc)
@@ -513,31 +559,22 @@ class SwiftlyCoreB200:
             torch.empty(shape, dtype=torch.complex128, device=b.device) if o is None else o
             for b, o in zip(BF_Fs, outs)
         ]
-        for lo in range(0, len(BF_Fs), 64):
-            chunk = range(lo, min(lo + 64, len(BF_Fs)))
-            din = (_lib.Lines * len(chunk))()
-            dout = (_lib.Lines * len(chunk))()
-            offs = (ctypes.c_int64 * len(chunk))()
-            for k, i in enumerate(chunk):
-                b, o = BF_Fs[i], outs[i]
-                self._check_tensor(b)
-                self._check_tensor(o)
-                if b.dtype != torch.complex128 or b.dim() != 2 or b.stride(1) != 1:
-                    raise ValueError("extract_columns needs row-contiguous complex128 tensors")
-                if b.shape[0] not in rows:
-                    raise ValueError(f"prepared facet has {b.shape[0]} rows, expected {rows[0]} "
-                                     f"(or a ring of {rows[1]}, or {rows[2]} half rows)!")
-                if tuple(o.shape) != shape or o.stride(1) != 1:
-                    raise ValueError(f"Output array has shape {tuple(o.shape)}, expected {shape}!")
-                din[k] = self._describe(b, 1)
-                dout[k] = self._describe(o, 1)
-                offs[k] = int(facet_off1s[i])
-            entry = (self._lib.swiftly_b200_extract_columns_windowed if prewindowed
-                     else self._lib.swiftly_b200_extract_columns)
-            rc = entry(self._plan, len(chunk), din, dout, int(subgrid_off0), offs,
-                       self._stream(BF_Fs[lo]))
-            _lib.check(self._lib, rc)
-        return outs
+
+        def chk_b(t):
+            if t.shape[0] not in rows:
+                raise ValueError(f"prepared facet has {t.shape[0]} rows, expected {rows[0]} "
+                                 f"(or a ring of {rows[1]}, or {rows[2]} half rows)!")
+
+        def chk_o(t):
+            if tuple(t.shape) != shape:
+                raise ValueError(f"Output array has shape {tuple(t.shape)}, expected {shape}!")
+
+        entry = (self._lib.swiftly_b200_extract_columns_windowed if prewindowed
+                 else self._lib.swiftly_b200_extract_columns)
+        return self._per_facet(
+            lambda n, din, dout, offs, _, stream: entry(
+                self._plan, n, din, dout, int(subgrid_off0), offs, stream),
+            BF_Fs, outs, facet_off1s, chk_b, chk_o)
 
     def sum_finish_axis_grouped(self, groups, out, axis, subgrid_off, mask=None):
         """:meth:`sum_finish_axis` for several source groups in ONE launch.
@@ -550,95 +587,31 @@ class SwiftlyCoreB200:
             different subgrids, e.g. a batch of the multi-GPU driver)
         :param mask: one mask (or None), or a list with one mask / None per group
         """
-        if isinstance(subgrid_off, (list, tuple)):
-            return self._sum_finish_axis_batched(groups, out, axis, subgrid_off, mask)
         if axis not in (0, 1):
             raise ValueError(f"Invalid axis {axis}")
-        self._check_tensor(out)
-        if out.dim() != 3 or out.shape[0] != len(groups):
-            raise ValueError("out must be (n_groups, lines, size) / (n_groups, size, lines)")
-        flat = [s for grp in groups for s in grp]
-        arr = (_lib.Source * max(1, len(flat)))()
-        other = 1 - axis
-        for i, (t, facet_off) in enumerate(flat):
-            self._check_tensor(t)
-            if t.dtype != torch.complex128 or t.dim() != 2:
-                raise ValueError("sources must be 2-D complex128 device tensors")
-            if t.shape[other] != out.shape[1 + other]:
-                raise ValueError(
-                    f"source has {t.shape[other]} lines, output {out.shape[1 + other]}")
-            arr[i] = _lib.Source(t.data_ptr(), t.stride(other), t.stride(axis), t.shape[axis],
-                                 int(facet_off))
-        sizes = (ctypes.c_int32 * len(groups))(*[len(g) for g in groups])
+        per_group = isinstance(subgrid_off, (list, tuple))
+        scattered = isinstance(out, (list, tuple))  # one output buffer per group
+        if not scattered:
+            self._check_tensor(out)
+            if out.dim() != 3:
+                raise ValueError("out must be (n_groups, lines, size) / (n_groups, size, lines)")
+        if (len(out) != len(groups) or (per_group and len(subgrid_off) != len(groups))
+                or (scattered and not per_group)):
+            raise ValueError("out / subgrid_off must have one entry per group")
         dout = self._describe(out[0], axis)
-        mptr = ctypes.c_void_p(0)
-        if mask is not None:
-            if mask.dtype != torch.float64 or mask.numel() != out.shape[1 + axis]:
-                raise ValueError("mask must be float64 of the subgrid size")
-            mask = mask.contiguous()
-            mptr = ctypes.c_void_p(mask.data_ptr())
+        if per_group:
+            block = PreparedSumFinish(self, groups, axis, dout.n_lines, dout.size,
+                                      (dout.line_stride, dout.elem_stride))
+            masks = [None] * len(groups) if mask is None else mask
+            if scattered:
+                block.launch(subgrid_off, masks, outs=out)
+                return list(out)
+            block.launch(subgrid_off, masks, out=out, out_group_stride=out.stride(0))
+            return out
+        arr, sizes, keep = self._sources(groups, axis, dout.n_lines)
         rc = self._lib.swiftly_b200_sum_finish_axis_grouped(
             self._plan, arr, sizes, len(groups), ctypes.byref(dout), int(out.stride(0)),
-            int(subgrid_off), mptr, self._stream(out))
-        _lib.check(self._lib, rc)
-        return out
-
-    def _sum_finish_axis_batched(self, groups, out, axis, subgrid_offs, masks):
-        if axis not in (0, 1):
-            raise ValueError(f"Invalid axis {axis}")
-        scattered = isinstance(out, (list, tuple))  # one output buffer per group
-        if scattered:
-            outs = list(out)
-            if len(outs) != len(groups) or len(subgrid_offs) != len(groups):
-                raise ValueError("out / subgrid_off must have one entry per group")
-            for o in outs:
-                self._check_tensor(o)
-                if (o.dim() != 2 or tuple(o.shape) != tuple(outs[0].shape)
-                        or o.stride() != outs[0].stride() or o.dtype != torch.complex128):
-                    raise ValueError("scattered outputs must share shape, strides and dtype")
-            out = outs[0][None]
-        self._check_tensor(out)
-        if out.dim() != 3 or (not scattered and out.shape[0] != len(groups)) \
-                or len(subgrid_offs) != len(groups):
-            raise ValueError("out / subgrid_off must have one entry per group")
-        if masks is None:
-            masks = [None] * len(groups)
-        flat = [s for grp in groups for s in grp]
-        arr = (_lib.Source * max(1, len(flat)))()
-        other = 1 - axis
-        for i, (t, facet_off) in enumerate(flat):
-            self._check_tensor(t)
-            if t.dtype != torch.complex128 or t.dim() != 2:
-                raise ValueError("sources must be 2-D complex128 device tensors")
-            if t.shape[other] != out.shape[1 + other]:
-                raise ValueError(
-                    f"source has {t.shape[other]} lines, output {out.shape[1 + other]}")
-            arr[i] = _lib.Source(t.data_ptr(), t.stride(other), t.stride(axis), t.shape[axis],
-                                 int(facet_off))
-        sizes = (ctypes.c_int32 * len(groups))(*[len(g) for g in groups])
-        offs = (ctypes.c_int64 * len(groups))(*[int(o) for o in subgrid_offs])
-        keep = []
-        mptrs = (ctypes.c_void_p * len(groups))()
-        for g, mk in enumerate(masks):
-            if mk is None:
-                mptrs[g] = None
-            else:
-                if mk.dtype != torch.float64 or mk.numel() != out.shape[1 + axis]:
-                    raise ValueError("mask must be float64 of the subgrid size")
-                mk = mk.contiguous()
-                keep.append(mk)
-                mptrs[g] = mk.data_ptr()
-        dout = self._describe(out[0], axis)
-        if scattered:
-            ptrs = (ctypes.c_void_p * len(groups))(*[o.data_ptr() for o in outs])
-            rc = self._lib.swiftly_b200_sum_finish_axis_scattered(
-                self._plan, arr, sizes, len(groups), ctypes.byref(dout), ptrs, offs, mptrs,
-                self._stream(outs[0]))
-            _lib.check(self._lib, rc)
-            return outs
-        rc = self._lib.swiftly_b200_sum_finish_axis_batched(
-            self._plan, arr, sizes, len(groups), ctypes.byref(dout), int(out.stride(0)),
-            offs, mptrs, self._stream(out))
+            int(subgrid_off), self._mask_ptr(mask, out, dout.size, keep), self._stream(out))
         _lib.check(self._lib, rc)
         return out
 
@@ -664,33 +637,16 @@ class SwiftlyCoreB200:
             contribution window for ``subgrid_off`` is cut on the fly) or
             ``xM_yN_size`` (already contributions)
         :param out: 2-D device tensor, ``axis`` of length subgrid size (overwritten)
-        :param mask: optional float64 device tensor of length subgrid size
+        :param mask: optional mask of length subgrid size
         """
         if axis not in (0, 1):
             raise ValueError(f"Invalid axis {axis}")
         self._check_tensor(out)
-        arr = (_lib.Source * len(sources))()
-        other = 1 - axis
-        for i, (t, facet_off) in enumerate(sources):
-            self._check_tensor(t)
-            if t.dtype != torch.complex128 or t.dim() != 2:
-                raise ValueError("sources must be 2-D complex128 device tensors")
-            if t.shape[other] != out.shape[other]:
-                raise ValueError(
-                    f"source has {t.shape[other]} lines, output {out.shape[other]}"
-                )
-            arr[i] = _lib.Source(t.data_ptr(), t.stride(other), t.stride(axis), t.shape[axis],
-                                 int(facet_off))
         dout = self._describe(out, axis)
-        mptr = ctypes.c_void_p(0)
-        if mask is not None:
-            if mask.dtype != torch.float64 or mask.numel() != out.shape[axis]:
-                raise ValueError("mask must be float64 of the subgrid size")
-            mask = mask.contiguous()
-            mptr = ctypes.c_void_p(mask.data_ptr())
+        arr, _, keep = self._sources([sources], axis, dout.n_lines)
         rc = self._lib.swiftly_b200_sum_finish_axis(
-            self._plan, arr, len(sources), ctypes.byref(dout), int(subgrid_off), mptr,
-            self._stream(out),
+            self._plan, arr, len(sources), ctypes.byref(dout), int(subgrid_off),
+            self._mask_ptr(mask, out, dout.size, keep), self._stream(out),
         )
         _lib.check(self._lib, rc)
         return out
@@ -704,7 +660,7 @@ class SwiftlyCoreB200:
         ``out[r, c] = m0[r] * m1[c] * src[r, c]`` is the subgrid of size ``sz`` at
         ``(off0, off1)``; ``mirror[r, c] = n0[r] * n1[c] * conj(src[2h - r, 2h - c])``,
         ``h = sz // 2``, the one at ``(-off0, -off1)``.  ``masks`` / ``mirror_masks``: None or
-        ``(mask0, mask1)``, each None or a float64 device tensor of ``sz`` samples.  ``out`` /
+        ``(mask0, mask1)``, each None or a mask of ``sz`` samples.  ``out`` /
         ``mirror`` may be given (any strides, e.g. views into larger arrays); device tensors only.
         """
         self._check_tensor(src)
@@ -720,18 +676,8 @@ class SwiftlyCoreB200:
                 raise ValueError(f"Output array has shape {tuple(t.shape)}, expected {shape}!")
             outs.append(t)
         keep = []
-        ptrs = []
-        for pair in (masks, mirror_masks):
-            for mk in (None, None) if pair is None else pair:
-                if mk is None:
-                    ptrs.append(None)
-                    continue
-                mk = mk.to(torch.float64).contiguous()
-                self._check_tensor(mk)
-                if mk.numel() != shape[0]:
-                    raise ValueError("mask must have the subgrid size")
-                keep.append(mk)
-                ptrs.append(mk.data_ptr())
+        ptrs = [self._mask_ptr(mk, outs[0], shape[0], keep)
+                for pair in (masks, mirror_masks) for mk in ((None, None) if pair is None else pair)]
         din, dout, dmir = (self._describe(t, 1) for t in (src, outs[0], outs[1]))
         rc = self._lib.swiftly_b200_mirror_subgrid(
             self._plan, ctypes.byref(din), ctypes.byref(dout), ctypes.byref(dmir), *ptrs,
@@ -796,11 +742,7 @@ class SwiftlyCoreB200:
             raise ValueError(f"Output array has shape {tuple(out.shape)} and dtype {out.dtype}, "
                              f"expected {shape} float64!")
         keep = []
-        mptr = ctypes.c_void_p(0)
-        if mask is not None:
-            mptr = self._mask_ptr(mask, out, keep)
-            if keep[0].numel() != shape[axis]:
-                raise ValueError("mask must have the facet size")
+        mptr = self._mask_ptr(mask, out, shape[axis], keep, "facet")
         other = 1 - axis
         dout = _lib.Lines(out.data_ptr(), shape[other], shape[axis], out.stride(other),
                           out.stride(axis), _lib.DEVICE)
@@ -906,6 +848,24 @@ class SwiftlyCoreB200:
             arr[k] = self._describe(t, 1)
         return arr
 
+    def _per_facet(self, call, ins, outs, offs, chk_in, chk_out, masks=None):
+        """``call(n, din, dout, offs, mptrs, stream)`` once per chunk of at most 64 facets
+        (``SW_MAX_COLUMN_FACETS``): the ``Lines`` of the chunk's ``ins`` and ``outs`` (row-contiguous
+        tensors checked by ``chk_in`` / ``chk_out``), its facet offsets and, with ``masks``, its
+        facet masks of ``outs[f].shape[1]`` samples (else ``mptrs`` is None).  Returns ``outs``."""
+        keep = []
+        for lo in range(0, len(ins), 64):
+            hi = min(lo + 64, len(ins))
+            din = self._lines_array(ins[lo:hi], chk_in)
+            dout = self._lines_array(outs[lo:hi], chk_out)
+            offs_k = (ctypes.c_int64 * (hi - lo))(*[int(o) for o in offs[lo:hi]])
+            mptrs = None if masks is None else (ctypes.c_void_p * (hi - lo))(*[
+                self._mask_ptr(mk, t, t.shape[1], keep, "facet")
+                for mk, t in zip(masks[lo:hi], outs[lo:hi])])
+            rc = call(hi - lo, din, dout, offs_k, mptrs, self._stream(ins[lo]))
+            _lib.check(self._lib, rc)
+        return outs
+
     def subgrid_to_facets(self, blocks, accs, facet_off1s, subgrid_off1):
         """One subgrid into the column accumulators of many facets, ONE launch per <= 64 facets.
 
@@ -923,15 +883,10 @@ class SwiftlyCoreB200:
             if tuple(t.shape) != (m, yN):
                 raise ValueError(f"accumulator has shape {tuple(t.shape)}, expected {(m, yN)}!")
 
-        for lo in range(0, len(blocks), 64):
-            hi = min(lo + 64, len(blocks))
-            din = self._lines_array(blocks[lo:hi], chk_b)
-            dout = self._lines_array(accs[lo:hi], chk_a)
-            offs = (ctypes.c_int64 * (hi - lo))(*[int(o) for o in facet_off1s[lo:hi]])
-            rc = self._lib.swiftly_b200_subgrid_to_facets(
-                self._plan, hi - lo, din, dout, offs, int(subgrid_off1), self._stream(accs[lo]))
-            _lib.check(self._lib, rc)
-        return accs
+        return self._per_facet(
+            lambda n, din, dout, offs, _, stream: self._lib.swiftly_b200_subgrid_to_facets(
+                self._plan, n, din, dout, offs, int(subgrid_off1), stream),
+            blocks, accs, facet_off1s, chk_b, chk_a)
 
     def fold_column(self, accs, facet_accs, facet_off1s, masks1, subgrid_off0):
         """Fold a finished subgrid column into many facet accumulators, ONE launch per <= 64.
@@ -941,8 +896,8 @@ class SwiftlyCoreB200:
         ``facet_accs[f]``: ``(yN_size, facet_size)``, added to; or, for every facet, an
         ``(xM_yN_size, facet_size)`` row ring holding row ``r`` of the column's window at line
         ``r mod xM_yN_size`` (include/swiftly_b200.h, "Row rings"), or every one holds the
-        ``yN_size // 2 + 1`` half rows of a real image ("Half rows"); ``masks1[f]``: float64
-        device tensor of the facet size or None.
+        ``yN_size // 2 + 1`` half rows of a real image ("Half rows"); ``masks1[f]``: a mask of
+        the facet size or None.
         """
         m, yN, half = self.xM_yN_size, self.yN_size, self.half_rows
 
@@ -955,32 +910,7 @@ class SwiftlyCoreB200:
                 raise ValueError(f"facet accumulator has {t.shape[0]} rows, expected {yN} "
                                  f"(or a ring of {m}, or {half} half rows)!")
 
-        keep = []
-        for lo in range(0, len(accs), 64):
-            hi = min(lo + 64, len(accs))
-            din = self._lines_array(accs[lo:hi], chk_a)
-            dout = (_lib.Lines * (hi - lo))()
-            for k, t in enumerate(facet_accs[lo:hi]):
-                self._check_tensor(t)
-                if t.dtype != torch.complex128 or t.dim() != 2 or t.stride(1) != 1:
-                    raise ValueError("need row-contiguous 2-D complex128 device tensors")
-                chk_f(t)
-                # lines = rows (yN of them), line length = facet size
-                dout[k] = _lib.Lines(t.data_ptr(), t.shape[0], t.shape[1], t.stride(0), 1,
-                                     _lib.DEVICE)
-            offs = (ctypes.c_int64 * (hi - lo))(*[int(o) for o in facet_off1s[lo:hi]])
-            mptrs = (ctypes.c_void_p * (hi - lo))()
-            for k, mk in enumerate(masks1[lo:hi]):
-                if mk is None:
-                    mptrs[k] = None
-                else:
-                    mk = mk.to(torch.float64).contiguous()
-                    if mk.numel() != facet_accs[lo + k].shape[1]:
-                        raise ValueError("mask must have the facet size")
-                    keep.append(mk)
-                    mptrs[k] = mk.data_ptr()
-            rc = self._lib.swiftly_b200_fold_column(
-                self._plan, hi - lo, din, dout, offs, mptrs, int(subgrid_off0),
-                self._stream(accs[lo]))
-            _lib.check(self._lib, rc)
-        return facet_accs
+        return self._per_facet(
+            lambda n, din, dout, offs, mptrs, stream: self._lib.swiftly_b200_fold_column(
+                self._plan, n, din, dout, offs, mptrs, int(subgrid_off0), stream),
+            accs, facet_accs, facet_off1s, chk_a, chk_f, masks1)
